@@ -74,7 +74,7 @@ __device__ __forceinline__ void tile_coords(int tile, const GemmArgs& g, int& m_
   n_blk = g.raster_n ? a : b;
 }
 
-// address of C[row, col] (a column pair never straddles a head)
+// address of C[row, col] (four adjacent columns from a multiple of 4 never straddle a head)
 __device__ __forceinline__ bf16* c_ptr(const GemmArgs& g, long long row, int col) {
   if (g.n_peers == 0) return g.C + row * g.ldc + col;
   const int t = col / g.peer_period, rem = col - t * g.peer_period;
@@ -97,6 +97,18 @@ __device__ __forceinline__ void store_pair(const GemmArgs& g, long long row, int
   }
   *reinterpret_cast<uint32_t*>(c_ptr(g, row, col)) = pack_bf16(v0, v1);
 }
+
+// Quad exchange for full-sector stores.  Lane q of a quad holds bf16 pairs `lo` (columns 8i + 2q + {0, 1}) and `hi` (columns
+// 8(i+1) + 2q + {0, 1}) of one row.  One shuffle leaves every lane four adjacent columns: even lanes 8i + 2q + {0..3}, odd lanes
+// 8(i+1) + 2(q-1) + {0..3} (`quad_cols` gives the offset from 8i).  A warp then writes each of its 8 rows as one whole 32-byte
+// sector with 8-byte stores, instead of two half-filled sectors with 4-byte stores.  Every lane of the warp must call it.
+__device__ __forceinline__ int quad_cols(int quad) { return (quad & 1) ? 8 + 2 * (quad - 1) : 2 * quad; }
+__device__ __forceinline__ uint2 quad_pair(uint32_t lo, uint32_t hi, int quad) {
+  const bool odd = quad & 1;
+  const uint32_t got = __shfl_xor_sync(0xffffffffu, odd ? lo : hi, 1);
+  return odd ? make_uint2(got, hi) : make_uint2(lo, got);
+}
+__device__ __forceinline__ void st_quad(bf16* p, uint2 v) { *reinterpret_cast<uint2*>(p) = v; }
 
 // fold (m2, s2, w2) into (m, s, w): running max, sum e^(x-max), sum e^(x-max) x
 __device__ __forceinline__ void lse_merge(float& m, float& s, float& w, float m2, float s2, float w2) {
@@ -208,44 +220,95 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         // the token's cos/sin row in fp32, one rounding on store -- the arithmetic of rotary_qk_kernel (elementwise.cu), which is
         // flash_attn's apply_rotary (layers/rotary.py:382-416, mha.py:648).
         const bool rotate = (long long)n_blk * BN < g.rope_cols;
+        const int qc = quad_cols(quad);
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
-          const long long row = row0 + 8 * h;
-          if (row >= g.M) continue;
+          const long long row = row0 + 8 * h;      // rows >= M (a ragged last block) compute and exchange, but store nothing
           const long long l = row % g.rope_L;
 #pragma unroll
           for (int hc = 0; hc < BN; hc += 128) {
 #pragma unroll
-            for (int i8 = 0; i8 < 8; ++i8) {
-              const int i = hc / 8 + i8, c = 8 * i8 + 2 * quad, col = n_blk * BN + hc + c;
-              const uint32_t b1 = ld_pair(g.bias + col), b2 = ld_pair(g.bias + col + 64);
-              const float x0 = rbf(acc[4 * i + 2 * h] + bf_lo(b1)), x1 = rbf(acc[4 * i + 2 * h + 1] + bf_hi(b1));
-              const float y0 = rbf(acc[4 * (i + 8) + 2 * h] + bf_lo(b2)), y1 = rbf(acc[4 * (i + 8) + 2 * h + 1] + bf_hi(b2));
-              uint32_t o1, o2;
-              if (rotate) {
-                const uint32_t cw2 = ld_pair(g.rope_cos + l * 64 + c), sw2 = ld_pair(g.rope_sin + l * 64 + c);
-                const float cl = bf_lo(cw2), ch = bf_hi(cw2), sl = bf_lo(sw2), sh = bf_hi(sw2);
-                o1 = pack_bf16(x0 * cl - y0 * sl, x1 * ch - y1 * sh);
-                o2 = pack_bf16(x0 * sl + y0 * cl, x1 * sh + y1 * ch);
-              } else {
-                o1 = pack_bf16(x0, x1); o2 = pack_bf16(y0, y1);
+            for (int i8 = 0; i8 < 8; i8 += 2) {
+              uint32_t o1[2], o2[2];
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                const int i = hc / 8 + i8 + e, c = 8 * (i8 + e) + 2 * quad, col = n_blk * BN + hc + c;
+                const uint32_t b1 = ld_pair(g.bias + col), b2 = ld_pair(g.bias + col + 64);
+                const float x0 = rbf(acc[4 * i + 2 * h] + bf_lo(b1)), x1 = rbf(acc[4 * i + 2 * h + 1] + bf_hi(b1));
+                const float y0 = rbf(acc[4 * (i + 8) + 2 * h] + bf_lo(b2)), y1 = rbf(acc[4 * (i + 8) + 2 * h + 1] + bf_hi(b2));
+                if (rotate) {
+                  const uint32_t cw2 = ld_pair(g.rope_cos + l * 64 + c), sw2 = ld_pair(g.rope_sin + l * 64 + c);
+                  const float cl = bf_lo(cw2), ch = bf_hi(cw2), sl = bf_lo(sw2), sh = bf_hi(sw2);
+                  o1[e] = pack_bf16(x0 * cl - y0 * sl, x1 * ch - y1 * sh);
+                  o2[e] = pack_bf16(x0 * sl + y0 * cl, x1 * sh + y1 * ch);
+                } else {
+                  o1[e] = pack_bf16(x0, x1); o2[e] = pack_bf16(y0, y1);
+                }
               }
-              *reinterpret_cast<uint32_t*>(c_ptr(g, row, col)) = o1;
-              *reinterpret_cast<uint32_t*>(c_ptr(g, row, col + 64)) = o2;
+              const uint2 w1 = quad_pair(o1[0], o1[1], quad), w2 = quad_pair(o2[0], o2[1], quad);
+              const int col = n_blk * BN + hc + 8 * i8 + qc;
+              if (row < g.M) { st_quad(c_ptr(g, row, col), w1); st_quad(c_ptr(g, row, col + 64), w2); }
             }
           }
         }
       } else if constexpr (EPI == EVO_EPI_GELU_GATE && BN == BN_BIG) {
         // packed [l1 | l2] tile: output column n_blk * 128 + c = bf16(gelu(bf16(l1))) * bf16(l2)
+        const int qc = quad_cols(quad);
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           const long long row = row0 + 8 * h;
-          if (row >= g.M) continue;
 #pragma unroll
-          for (int i = 0; i < BN / 16; ++i) {
-            const float a0 = rbf(acc[4 * i + 2 * h]), a1 = rbf(acc[4 * i + 2 * h + 1]);
-            const float b0 = rbf(acc[4 * (i + BN / 16) + 2 * h]), b1 = rbf(acc[4 * (i + BN / 16) + 2 * h + 1]);
-            *reinterpret_cast<uint32_t*>(c_ptr(g, row, n_blk * (BN / 2) + 8 * i + 2 * quad)) = pack_bf16(rbf(gelu_erf(a0)) * b0, rbf(gelu_erf(a1)) * b1);
+          for (int i = 0; i < BN / 16; i += 2) {
+            uint32_t o[2];
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const float a0 = rbf(acc[4 * (i + e) + 2 * h]), a1 = rbf(acc[4 * (i + e) + 2 * h + 1]);
+              const float b0 = rbf(acc[4 * (i + e + BN / 16) + 2 * h]), b1 = rbf(acc[4 * (i + e + BN / 16) + 2 * h + 1]);
+              o[e] = pack_bf16(rbf(gelu_erf(a0)) * b0, rbf(gelu_erf(a1)) * b1);
+            }
+            const uint2 w = quad_pair(o[0], o[1], quad);
+            if (row < g.M) st_quad(c_ptr(g, row, n_blk * (BN / 2) + 8 * i + qc), w);
+          }
+        }
+      } else if constexpr (BN == BN_BIG) {
+        // bias, then the bf16 rounding of the linear output (exact in the exchanged bf16 pairs), then the residual.  The residual
+        // of half a row is loaded ahead of its stores (one load latency per half row, not one per column pair); C may alias it,
+        // since every element is read before the same thread writes it.
+        constexpr bool BIAS = EPI == EVO_EPI_BIAS || EPI == EVO_EPI_BIAS_RESID, RESID = EPI == EVO_EPI_BIAS_RESID || EPI == EVO_EPI_RESID;
+        const int qc = quad_cols(quad);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const long long row = row0 + 8 * h;
+          const bool live = row < g.M;
+          constexpr int CH = BN / 32;              // residual words loaded ahead per chunk (half a row: no register spills)
+#pragma unroll
+          for (int i0 = 0; i0 < BN / 16; i0 += CH) {
+            uint2 r[CH];
+            if constexpr (RESID) {
+#pragma unroll
+              for (int j = 0; j < CH; ++j)
+                r[j] = live ? __ldg(reinterpret_cast<const uint2*>(g.resid + row * g.ldr + n_blk * BN + 16 * (i0 + j) + qc)) : make_uint2(0u, 0u);
+            }
+#pragma unroll
+            for (int j = 0; j < CH; ++j) {
+              const int i = i0 + j;
+              uint32_t o[2];
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                float v0 = acc[4 * (2 * i + e) + 2 * h], v1 = acc[4 * (2 * i + e) + 2 * h + 1];
+                if constexpr (BIAS) {
+                  const uint32_t b = ld_pair(g.bias + n_blk * BN + 8 * (2 * i + e) + 2 * quad);
+                  v0 += bf_lo(b); v1 += bf_hi(b);
+                }
+                o[e] = pack_bf16(v0, v1);
+              }
+              uint2 w = quad_pair(o[0], o[1], quad);
+              if constexpr (RESID) {
+                w.x = pack_bf16(bf_lo(w.x) + bf_lo(r[j].x), bf_hi(w.x) + bf_hi(r[j].x));
+                w.y = pack_bf16(bf_lo(w.y) + bf_lo(r[j].y), bf_hi(w.y) + bf_hi(r[j].y));
+              }
+              if (live) st_quad(c_ptr(g, row, n_blk * BN + 16 * i + qc), w);
+            }
           }
         }
       } else {
