@@ -28,15 +28,17 @@ __global__ void gelu_gate_kernel(const bf16* __restrict__ t, bf16* __restrict__ 
   *reinterpret_cast<uint32_t*>(out + m * ipad + c2) = pack_bf16(o0, o1);
 }
 
-// L == 1: rotary on q,k at position *pos, k,v appended to the cache at row *pos.
+// L == 1: rotary on q,k at position pos_ptr[b * pos_stride], k,v appended to the cache at that row.  pos_stride 0 = one
+// position shared by the batch, 1 = one position per row (prompts of different lengths decoded together).
 // qkv (B, 3, H, 128) in place; cos/sin tables indexed by absolute position.
 __global__ void decode_qkv_prep_kernel(bf16* __restrict__ qkv, bf16* __restrict__ cache, const bf16* __restrict__ cos, const bf16* __restrict__ sin,
-                                       const long long* __restrict__ pos_ptr, int B, int H, long long max_seqlen) {
+                                       const long long* __restrict__ pos_ptr, int pos_stride, int B, int H, long long max_seqlen) {
   pdl_launch_dependents(); pdl_wait();
-  const long long pos = *pos_ptr;
   int idx = blockIdx.x * blockDim.x + threadIdx.x;       // (b, h, i) i in [0, 64)
-  if (idx >= B * H * 64 || pos >= max_seqlen) return;
+  if (idx >= B * H * 64) return;
   int i = idx % 64, h = (idx / 64) % H, b = idx / (64 * H);
+  const long long pos = pos_ptr[(long long)b * pos_stride];
+  if (pos >= max_seqlen) return;
   const float c = __bfloat162float(cos[pos * 64 + i]), s = __bfloat162float(sin[pos * 64 + i]);
   bf16* q = qkv + ((long long)(b * 3 + 0) * H + h) * HD;
   bf16* k = qkv + ((long long)(b * 3 + 1) * H + h) * HD;
@@ -53,17 +55,17 @@ __global__ void decode_qkv_prep_kernel(bf16* __restrict__ qkv, bf16* __restrict_
   cv[i] = v[i]; cv[i + 64] = v[i + 64];
 }
 
-// Single-query attention over the KV cache, keys [0, *pos].  grid (H, B, nsplit); each CTA scans a
+// Single-query attention over the KV cache, keys [0, pos_ptr[b * pos_stride]].  grid (H, B, nsplit); each CTA scans a
 // contiguous key range: thread t owns keys t, t+128, ... of the range (one 256-byte K row and one
 // V row per key), keeps an online-softmax state and a 128-wide fp32 accumulator in registers, and the
 // 128 partial states are merged through shared memory; splits are merged by the last kernel.
 constexpr int DT = 128;
 __global__ void __launch_bounds__(DT) decode_attn_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ cache, float* __restrict__ part_o,
-                                                         float* __restrict__ part_ml, const long long* __restrict__ pos_ptr,
+                                                         float* __restrict__ part_ml, const long long* __restrict__ pos_ptr, int pos_stride,
                                                          int H, long long max_seqlen, int nsplit, float scale) {
   pdl_launch_dependents(); pdl_wait();
   const int h = blockIdx.x, b = blockIdx.y, sp = blockIdx.z, tid = threadIdx.x;
-  const long long nk = min(*pos_ptr + 1, max_seqlen);
+  const long long nk = min(pos_ptr[(long long)b * pos_stride] + 1, max_seqlen);   // per row: a split past the row's keys stays empty
   const long long per = (nk + nsplit - 1) / nsplit;
   const long long k0 = (long long)sp * per, k1 = min(nk, k0 + per);
   __shared__ float qs[HD];
@@ -141,7 +143,8 @@ constexpr int TILE_BYTES = TK * HD * 2;          // 16 KB (K) + 16 KB (V) per st
 constexpr int ATT2_SMEM = AST * 2 * TILE_BYTES + 1024;
 __global__ void __launch_bounds__(160, 2) decode_attn_tma_kernel(const __grid_constant__ CUtensorMap tm, const bf16* __restrict__ qkv,
                                                                  float* __restrict__ part_o, float* __restrict__ part_ml,
-                                                                 const long long* __restrict__ pos_ptr, int H, long long S, int nsplit, float scale) {
+                                                                 const long long* __restrict__ pos_ptr, int pos_stride, int H, long long S, int nsplit,
+                                                                 float scale) {
   pdl_launch_dependents(); pdl_wait();
   extern __shared__ __align__(1024) uint8_t smem[];
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + AST * 2 * TILE_BYTES);
@@ -149,7 +152,7 @@ __global__ void __launch_bounds__(160, 2) decode_attn_tma_kernel(const __grid_co
   bf16* qb = reinterpret_cast<bf16*>(empty + AST);                   // 256 B
   float* red = reinterpret_cast<float*>(qb + HD);                      // [4][2] (m, l) then [4][128] o, overlaid on stage 0 after the loop
   const int h = blockIdx.x, b = blockIdx.y, sp = blockIdx.z, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const long long nk = min(*pos_ptr + 1, S);
+  const long long nk = min(pos_ptr[(long long)b * pos_stride] + 1, S);   // keys, splits and tiles are per row
   long long per = (nk + nsplit - 1) / nsplit;
   per = (per + TK - 1) / TK * TK;                                      // splits start on tile boundaries
   const long long k0 = (long long)sp * per, k1 = min(nk, k0 + per);
@@ -265,6 +268,12 @@ __global__ void decode_attn_merge_kernel(const float* __restrict__ part_o, const
 
 __global__ void add_i64_kernel(long long* p, long long v) { *p += v; }
 
+__global__ void add_i64_rows_kernel(long long* p, int n, long long v) {
+  pdl_launch_dependents(); pdl_wait();
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) p[i] += v;
+}
+
 }  // namespace
 
 extern "C" int evo_gelu_gate_interleaved(const void* t, void* out, int64_t M, int ipad, void* stream) {
@@ -275,50 +284,73 @@ extern "C" int evo_gelu_gate_interleaved(const void* t, void* out, int64_t M, in
   return check_launch("evo_gelu_gate_interleaved");
 }
 
-extern "C" int evo_decode_qkv_prep(void* qkv, void* cache, const void* cos, const void* sin, const int64_t* pos,
-                                   int B, int H, int hd, int64_t max_seqlen, void* stream) {
-  EVO_REQUIRE(hd == HD, "evo_decode_qkv_prep: head_dim %d unsupported", hd);
+static int decode_qkv_prep(const char* what, void* qkv, void* cache, const void* cos, const void* sin, const int64_t* pos, int pos_stride,
+                           int B, int H, int hd, int64_t max_seqlen, void* stream) {
+  EVO_REQUIRE(hd == HD, "%s: head_dim %d unsupported", what, hd);
   int n = B * H * 64;
   EVO_CUDA(launch_pdl(decode_qkv_prep_kernel, dim3((n + 127) / 128), dim3(128), 0, (cudaStream_t)stream, (bf16*)qkv, (bf16*)cache, (const bf16*)cos, (const bf16*)sin,
-                      (const long long*)pos, B, H, max_seqlen));
-  return check_launch("evo_decode_qkv_prep");
+                      (const long long*)pos, pos_stride, B, H, max_seqlen));
+  return check_launch(what);
+}
+
+extern "C" int evo_decode_qkv_prep(void* qkv, void* cache, const void* cos, const void* sin, const int64_t* pos,
+                                   int B, int H, int hd, int64_t max_seqlen, void* stream) {
+  return decode_qkv_prep("evo_decode_qkv_prep", qkv, cache, cos, sin, pos, 0, B, H, hd, max_seqlen, stream);
+}
+
+extern "C" int evo_decode_qkv_prep_rows(void* qkv, void* cache, const void* cos, const void* sin, const int64_t* pos,
+                                        int B, int H, int hd, int64_t max_seqlen, void* stream) {
+  return decode_qkv_prep("evo_decode_qkv_prep_rows", qkv, cache, cos, sin, pos, 1, B, H, hd, max_seqlen, stream);
 }
 
 extern "C" size_t evo_decode_attn_workspace(int B, int H, int nsplit) { return (size_t)B * H * nsplit * (HD + 2) * sizeof(float); }
 
-extern "C" int evo_decode_attn(const void* qkv, const void* cache, void* out, const int64_t* pos, int B, int H, int hd,
-                               int64_t max_seqlen, int nsplit, float softmax_scale, void* workspace, size_t workspace_bytes, void* stream) {
-  EVO_REQUIRE(hd == HD, "evo_decode_attn: head_dim %d unsupported", hd);
-  EVO_REQUIRE(nsplit >= 1 && nsplit <= 64, "evo_decode_attn: bad nsplit %d", nsplit);
-  EVO_REQUIRE(workspace && workspace_bytes >= evo_decode_attn_workspace(B, H, nsplit), "evo_decode_attn: workspace too small");
+static int decode_attn(const char* what, const void* qkv, const void* cache, void* out, const int64_t* pos, int pos_stride, int B, int H, int hd,
+                       int64_t max_seqlen, int nsplit, float softmax_scale, void* workspace, size_t workspace_bytes, void* stream) {
+  EVO_REQUIRE(hd == HD, "%s: head_dim %d unsupported", what, hd);
+  EVO_REQUIRE(nsplit >= 1 && nsplit <= 64, "%s: bad nsplit %d", what, nsplit);
+  EVO_REQUIRE(workspace && workspace_bytes >= evo_decode_attn_workspace(B, H, nsplit), "%s: workspace too small", what);
   float* part_o = (float*)workspace;
   float* part_ml = part_o + (size_t)B * H * nsplit * HD;
   static const bool force_v1 = getenv("EVO_B200_DECODE_ATTN_V1") != nullptr;
+  int rc;
   if (max_seqlen % TK == 0 && !force_v1 && (long long)B * max_seqlen < (1LL << 31)) {
     CUtensorMap tm;
     const uint64_t dims[3] = {(uint64_t)HD, (uint64_t)(2 * H), (uint64_t)B * (uint64_t)max_seqlen};
     const uint64_t str[2] = {(uint64_t)HD * 2, (uint64_t)2 * H * HD * 2};
     const uint32_t box[3] = {(uint32_t)HD, 1, (uint32_t)TK};
-    int rc = make_tmap_nd_bf16(&tm, cache, 3, dims, str, box, false);
+    rc = make_tmap_nd_bf16(&tm, cache, 3, dims, str, box, false);
     if (rc) return rc;
     static unsigned long long attr_done = 0;
     if ((rc = ensure_dyn_smem(decode_attn_tma_kernel, ATT2_SMEM, attr_done))) return rc;
     EVO_CUDA(launch_pdl(decode_attn_tma_kernel, dim3(H, B, nsplit), dim3(160), (size_t)ATT2_SMEM, (cudaStream_t)stream, tm, (const bf16*)qkv, part_o, part_ml,
-                        (const long long*)pos, H, (long long)max_seqlen, nsplit, softmax_scale));
-    rc = check_launch("evo_decode_attn");
-    if (rc) return rc;
-    EVO_CUDA(launch_pdl(decode_attn_merge_kernel, dim3(H, B), dim3(HD), 0, (cudaStream_t)stream, (const float*)part_o, (const float*)part_ml, (bf16*)out, H, nsplit));
-    return check_launch("evo_decode_attn_merge");
+                        (const long long*)pos, pos_stride, H, (long long)max_seqlen, nsplit, softmax_scale));
+  } else {
+    EVO_CUDA(launch_pdl(decode_attn_kernel, dim3(H, B, nsplit), dim3(DT), 0, (cudaStream_t)stream, (const bf16*)qkv, (const bf16*)cache, part_o, part_ml,
+                        (const long long*)pos, pos_stride, H, max_seqlen, nsplit, softmax_scale));
   }
-  EVO_CUDA(launch_pdl(decode_attn_kernel, dim3(H, B, nsplit), dim3(DT), 0, (cudaStream_t)stream, (const bf16*)qkv, (const bf16*)cache, part_o, part_ml,
-                      (const long long*)pos, H, max_seqlen, nsplit, softmax_scale));
-  int rc = check_launch("evo_decode_attn");
-  if (rc) return rc;
+  if ((rc = check_launch(what))) return rc;
   EVO_CUDA(launch_pdl(decode_attn_merge_kernel, dim3(H, B), dim3(HD), 0, (cudaStream_t)stream, (const float*)part_o, (const float*)part_ml, (bf16*)out, H, nsplit));
   return check_launch("evo_decode_attn_merge");
+}
+
+extern "C" int evo_decode_attn(const void* qkv, const void* cache, void* out, const int64_t* pos, int B, int H, int hd,
+                               int64_t max_seqlen, int nsplit, float softmax_scale, void* workspace, size_t workspace_bytes, void* stream) {
+  return decode_attn("evo_decode_attn", qkv, cache, out, pos, 0, B, H, hd, max_seqlen, nsplit, softmax_scale, workspace, workspace_bytes, stream);
+}
+
+extern "C" int evo_decode_attn_rows(const void* qkv, const void* cache, void* out, const int64_t* pos, int B, int H, int hd,
+                                    int64_t max_seqlen, int nsplit, float softmax_scale, void* workspace, size_t workspace_bytes, void* stream) {
+  return decode_attn("evo_decode_attn_rows", qkv, cache, out, pos, 1, B, H, hd, max_seqlen, nsplit, softmax_scale, workspace, workspace_bytes, stream);
 }
 
 extern "C" int evo_advance_position(int64_t* pos, int64_t delta, void* stream) {
   add_i64_kernel<<<1, 1, 0, (cudaStream_t)stream>>>((long long*)pos, delta);
   return check_launch("evo_advance_position");
+}
+
+extern "C" int evo_advance_positions(int64_t* pos, int B, int64_t delta, void* stream) {
+  EVO_REQUIRE(B >= 1, "evo_advance_positions: bad batch %d", B);
+  EVO_CUDA(launch_pdl(add_i64_rows_kernel, dim3((B + 127) / 128), dim3(128), 0, (cudaStream_t)stream, (long long*)pos, B, (long long)delta));
+  return check_launch("evo_advance_positions");
 }

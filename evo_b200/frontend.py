@@ -89,6 +89,22 @@ def length_buckets(seqs: Sequence[str], batch_size: int = 32, mode: str = "exact
     return out
 
 
+def ragged_batches(lengths: Sequence[int], n_new: int, batch_size: int = 64, align: int = 64) -> List[Tuple[List[int], int]]:
+    """Plan of ragged generation: [(row indices, KV-cache length)] per decode batch.  Indices are sorted by (length, index),
+    so prompts of equal length are adjacent rows (what StripedHyena.prefill_ragged needs), and cut into batches of at most
+    `batch_size`; a batch's cache holds its longest prompt plus `n_new` tokens, rounded up to `align` (64: the length the
+    TMA-fed decode attention takes)."""
+    if batch_size < 1:
+        raise ValueError("batch_size must be >= 1")
+    order = sorted(range(len(lengths)), key=lambda i: (lengths[i], i))
+    out = []
+    for k in range(0, len(order), batch_size):
+        rows = order[k:k + batch_size]
+        need = lengths[rows[-1]] + n_new
+        out.append((rows, (need + align - 1) // align * align))
+    return out
+
+
 # ----------------------------------------------------------------------------- host bytes -> device ids
 def device_batch(seqs: Sequence[str], tokenizer: CharLevelTokenizer, prepend_bos: bool = True, device: str = "cuda:0",
                  dtype: torch.dtype = torch.long) -> Tuple[torch.Tensor, List[int]]:

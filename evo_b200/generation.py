@@ -183,14 +183,77 @@ class Generator:
         return picked[:, :done], kept_logits[:, :done], state
 
 
+def _generate_ragged(prompt_seqs, model, tokenizer, engine, n_tokens, prepend_bos, batch_size, verbose):
+    """generate(ragged=True): prompts sorted by length and cut into batches of <= batch_size; per batch one ragged prefill
+    (StripedHyena.prefill_ragged), one first pick (evo_sample) and one on-device loop with per-row positions.  Texts and
+    scores come back in input order."""
+    from . import _lib
+    from .frontend import ragged_batches
+    if n_tokens < 1:
+        raise ValueError("ragged generation needs n_tokens >= 1")
+    if not hasattr(model, "prefill_ragged"):
+        raise ValueError("ragged generation needs the evo_b200 StripedHyena model")
+    p0 = next(model.parameters(), None)
+    if p0 is None or p0.device.type != "cuda":
+        raise ValueError("ragged generation runs on CUDA only: move the model with .to('cuda:N')")
+    ids = [([tokenizer.eod_id] if prepend_bos else []) + tokenizer.tokenize(p) for p in prompt_seqs]
+    if any(len(p) == 0 for p in prompt_seqs):
+        raise ValueError("ragged generation: empty prompt")
+    limit = model.config.get("max_seqlen") or 8192
+    too_long = [i for i, t in enumerate(ids) if len(t) > limit]
+    if too_long:
+        raise _lib.EvoError(f"prompt {too_long[0]} has {len(ids[too_long[0]])} tokens, above the model's max_seqlen {limit}")
+    dev = p0.device
+    V = tokenizer.vocab_size
+    texts: List[str] = [""] * len(ids)
+    scores: List[float] = [0.0] * len(ids)
+    pick_args = dict(top_k=engine.top_k, top_p=engine.top_p, temperature=engine.temperature)
+    for rows, cache_len in ragged_batches([len(t) for t in ids], n_tokens, batch_size):
+        picked = torch.empty(len(rows), n_tokens, dtype=torch.long, device=dev)
+        kept_logits = torch.empty(len(rows), n_tokens, V, dtype=torch.float, device=dev)
+        with torch.inference_mode():
+            head, state = model.prefill_ragged([ids[r] for r in rows], cache_len)
+        token = engine._pick_device(head)
+        kept_logits[:, 0], picked[:, 0] = head, token
+        if n_tokens > 1:
+            start = torch.tensor([len(ids[r]) for r in rows], dtype=torch.int64)
+            got, got_logits = model.decode_loop(token, state, n_tokens - 1, start, n_out=n_tokens - 1, **pick_args)
+            picked[:, 1:], kept_logits[:, 1:] = got, got_logits
+        del state, head
+        if verbose > 1:
+            print(f"[generate] ragged batch of {len(rows)}: prompt lengths {len(ids[rows[0]])}..{len(ids[rows[-1]])}, cache {cache_len}")
+        decoded = tokenizer.detokenize_batch(picked)
+        # logits_to_logprobs(trim_bos=True) pairs logits[i] with token[i+1]: the reference's alignment (Q3)
+        per_token = logits_to_logprobs(kept_logits, picked).float().cpu().numpy()
+        for k, r in enumerate(rows):
+            texts[r], scores[r] = decoded[k], float(np.mean(per_token[k]))
+    return texts, scores
+
+
 def generate(prompt_seqs: List[str], model, tokenizer: CharLevelTokenizer, n_tokens: int = 100, temperature: float = 0.0,
              top_k: int = 1, top_p: float = 1.0, batched: bool = True, prepend_bos: bool = False,
              cached_generation: bool = False, force_prompt_threshold: int = 128, verbose: int = 1,
-             device: str = "cuda:0", **kwargs) -> Tuple[List[str], List[float]]:
+             device: str = "cuda:0", ragged: bool = False, batch_size: int = 64, **kwargs) -> Tuple[List[str], List[float]]:
     """Sequences and mean log-likelihood "scores" for a list of prompts.  Prompts of one common
-    length run as one batch; anything else falls back to one prompt at a time (with a note on stderr)."""
+    length run as one batch; anything else falls back to one prompt at a time (with a note on stderr).
+
+    ragged=True batches prompts of different lengths: they are sorted by length and cut into batches of at most
+    `batch_size` (64 keeps the stream-K decode GEMMs; larger batches take the 128x64 tiles), and each batch decodes with a
+    position per row.  Every prompt is prefilled whole, so `force_prompt_threshold` does not apply and the reference's
+    jump to the full prompt length (Q1) never happens.  Needs cached_generation=True, a CUDA model, non-empty prompts no
+    longer than the model's max_seqlen, and n_tokens >= 1; texts and scores come back in input order."""
     model.eval()
     engine = Generator(model, tokenizer, top_k=top_k, top_p=top_p, temperature=temperature)
+    if ragged:
+        if not cached_generation:
+            raise ValueError("ragged generation needs cached_generation=True")
+        if batch_size < 1:
+            raise ValueError("batch_size must be >= 1")
+        texts, scores = _generate_ragged(list(prompt_seqs), model, tokenizer, engine, int(n_tokens), prepend_bos, int(batch_size), verbose)
+        if verbose:
+            for prompt, text, score in zip(prompt_seqs, texts, scores):
+                print(f'Prompt: "{prompt}",\tOutput: "{text}",\tScore: {score}')
+        return texts, scores
     uniform = len({len(p) for p in prompt_seqs}) <= 1
     if batched and uniform:
         work = [list(prompt_seqs)]

@@ -579,16 +579,17 @@ class StripedHyena(nn.Module):
         self._tiled = t
         return t
 
-    def _decode_body(self, x, pos_dev, ipd, B):
-        """One token per sequence through all blocks; every launch reads the position from pos_dev."""
+    def _decode_body(self, x, pos_dev, ipd, B, per_row=False):
+        """One token per sequence through all blocks; every launch reads the position from pos_dev: one shared int64, or
+        (per_row) one per row, pos_dev[b] for row b (the _rows entry points)."""
         lib = _lib.lib()
         prev = lib.evo_set_pdl(int(self.decode_pdl))
         try:
-            return self._decode_body_impl(x, pos_dev, ipd, B)
+            return self._decode_body_impl(x, pos_dev, ipd, B, per_row)
         finally:
             lib.evo_set_pdl(prev)
 
-    def _decode_body_impl(self, x, pos_dev, ipd, B):
+    def _decode_body_impl(self, x, pos_dev, ipd, B, per_row=False):
         cfg = self.config
         d, H, V = cfg.hidden_size, cfg.num_attention_heads, cfg.vocab_size
         hd = d // H
@@ -599,6 +600,8 @@ class StripedHyena(nn.Module):
         tiled = self._ensure_tiled() if (self.decode_tiled and not streamk) else None
         G2 = 3 if tiled is not None else 2       # weight-streaming tiles (3: tile-major weights)
         wsel = (lambda i, name, w: tiled[i][name]) if tiled is not None else (lambda i, name, w: w)
+        qkv_prep = lib.evo_decode_qkv_prep_rows if per_row else lib.evo_decode_qkv_prep
+        decode_attn = lib.evo_decode_attn_rows if per_row else lib.evo_decode_attn
 
         def lin(a, w, out, N, K, epi, bias=None, resid=None):
             if streamk:
@@ -619,11 +622,11 @@ class StripedHyena(nn.Module):
                 lin(xn, wsel(i, "in", mha.Wqkv.weight), qkv, 3 * d, d, EPI_BIAS if mha.Wqkv.bias is not None else EPI_NONE, bias=mha.Wqkv.bias)
                 cache = mha_ip.key_value_memory_dict[i]
                 cos, sin = self._rope_tables(cache.shape[1], dev)
-                check(lib.evo_decode_qkv_prep(ptr(qkv), ptr(cache), ptr(cos), ptr(sin), ptr(pos_dev), B, H, hd, cache.shape[1], self._stream()), "evo_decode_qkv_prep")
+                check(qkv_prep(ptr(qkv), ptr(cache), ptr(cos), ptr(sin), ptr(pos_dev), B, H, hd, cache.shape[1], self._stream()), "evo_decode_qkv_prep")
                 nws = lib.evo_decode_attn_workspace(B, H, nsplit)
                 ws = torch.empty(nws, dtype=torch.uint8, device=dev)
                 ctx = xn
-                check(lib.evo_decode_attn(ptr(qkv), ptr(cache), ptr(ctx), ptr(pos_dev), B, H, hd, cache.shape[1], nsplit,
+                check(decode_attn(ptr(qkv), ptr(cache), ptr(ctx), ptr(pos_dev), B, H, hd, cache.shape[1], nsplit,
                                           1.0 / math.sqrt(hd), ptr(ws), nws, self._stream()), "evo_decode_attn")
                 lin(ctx, wsel(i, "out", mha.out_proj.weight), u2, d, d, EPI_BIAS_RESID if mha.out_proj.bias is not None else EPI_RESID,
                     bias=mha.out_proj.bias, resid=u)
@@ -662,16 +665,66 @@ class StripedHyena(nn.Module):
         lin(u, tiled["unembed"] if tiled is not None else self.unembed.weight, logits, V, d, EPI_NONE)
         return logits
 
+    # ---- prefill of prompts of different lengths into one decode batch ------------------------------------------------
+    def prefill_ragged(self, prompts, cache_len):
+        """Prefill B prompts of different lengths into one state that decode_loop steps with per-row positions.
+
+        prompts: B non-empty 1-D token sequences (lists or int tensors); rows of equal length must be adjacent (sort by
+        length).  The rows are grouped by exact length (frontend.length_buckets) and each group runs the stateful forward
+        once.  Every attention layer gets one (B, cache_len, 2, H, 128) KV cache; a group's InferenceParams holds its row
+        slice cache[r0:r1], which is contiguous (the cache is batch-major), so the prefill writes and reads it in place.
+        The groups' Hyena states are concatenated along the batch.  No row is padded: each row's state is its own prefill's.
+        Returns (head (B, V) bf16: each row's logits at its last prompt position, the inference params dict).  Step 0 of
+        decode_loop then runs at start_pos = the prompt lengths."""
+        from ..frontend import length_buckets
+        cfg = self.config
+        B = len(prompts)
+        lengths = [len(p) for p in prompts]
+        if B == 0 or min(lengths) == 0:
+            raise ValueError("prefill_ragged needs at least one prompt and no empty prompt")
+        if max(lengths) > cache_len:
+            raise _lib.EvoError(f"prompt length {max(lengths)} exceeds the KV cache ({cache_len})")
+        groups = length_buckets(prompts, batch_size=B, mode="exact")
+        for idx in groups:
+            if idx != list(range(idx[0], idx[0] + len(idx))):
+                raise ValueError("prefill_ragged: prompts of equal length must be adjacent rows (sort the prompts by length)")
+        self._ensure_packed()
+        dev = self.embedding_layer.weight.device
+        d, H, V = cfg.hidden_size, cfg.num_attention_heads, cfg.vocab_size
+        with torch.cuda.device(dev), torch.no_grad():
+            caches = {i: torch.zeros(B, cache_len, 2, H, d // H, dtype=torch.bfloat16, device=dev) for i in sorted(self._attn_idxs)}
+            head = torch.empty(B, V, dtype=torch.bfloat16, device=dev)
+            fir, state = {}, {}
+            for idx in sorted(groups, key=lambda g: g[0]):
+                r0, r1 = idx[0], idx[-1] + 1
+                ids = torch.stack([torch.as_tensor(prompts[r], dtype=torch.long).to(dev) for r in idx])
+                ip = {"mha": InferenceParams(max_seqlen=cache_len, max_batch_size=r1 - r0, seqlen_offset=0,
+                                             key_value_memory_dict={i: c[r0:r1] for i, c in caches.items()}),
+                      "hyena": RecurrentInferenceParams(fir_filter_length=cfg.short_filter_length, state_dim=cfg.state_size, seqlen_offset=0)}
+                logits, ip = self.forward(ids, inference_params_dict=ip)
+                head[r0:r1] = logits[:, -1]
+                for i in ip["hyena"].state_dict:
+                    state.setdefault(i, []).append(ip["hyena"].state_dict[i])
+                    fir.setdefault(i, []).append(ip["hyena"].fir_state_dict[i])
+            hy = RecurrentInferenceParams(fir_filter_length=cfg.short_filter_length, state_dim=cfg.state_size, seqlen_offset=0)
+            hy.state_dict = {i: torch.cat(v, 0) for i, v in state.items()}
+            hy.fir_state_dict = {i: torch.cat(v, 0) for i, v in fir.items()}
+            mha = InferenceParams(max_seqlen=cache_len, max_batch_size=B, seqlen_offset=0, key_value_memory_dict=caches,
+                                  lengths_per_sample=torch.tensor(lengths, dtype=torch.int64, device=dev))
+        return head, {"mha": mha, "hyena": hy}
+
     # ---- on-device generation loop (SURVEY 8f-2): token pick + bookkeeping + feedback inside the captured step ------
     def decode_loop(self, first_token, ipd, n_steps, start_pos, *, top_k=1, top_p=0.0, temperature=1.0, forced=None, n_out=None, seed=None):
         """Run `n_steps` single-token steps without returning to the host in between.
 
         first_token (B,) or (B, 1): the input of step 0; ipd: populated state (after a prefill); start_pos: sequence
-        position of step 0 (the reference sets the FULL prompt length here, evo/generation.py:143).  Step i feeds the
+        position of step 0 (the reference sets the FULL prompt length here, evo/generation.py:143), an int shared by every
+        row, or a (B,) int64 tensor of per-row positions (prompts of different lengths, see prefill_ragged).  Step i feeds the
         token of step i-1; the token of step i is forced[:, i] while i < forced.shape[1] (teacher-forced prompt tail,
         evo/generation.py:156-160), afterwards it is picked on the device by evo_sample_step.
         Returns (picked (B, n_out) int64, kept_logits (B, n_out, V) fp32) for the sampled steps; the state holders'
-        seqlen_offset end at the value the per-token protocol would leave.
+        seqlen_offset end at the value the per-token protocol would leave (per-row positions: the largest row's, and the
+        attention holder's lengths_per_sample holds every row's).
         One CUDA graph = one whole step (all blocks + sampler + counters); the host only replays it."""
         lib = _lib.lib()
         dev = self.embedding_layer.weight.device
@@ -685,9 +738,19 @@ class StripedHyena(nn.Module):
         n_out = n_steps - n_forced if n_out is None else n_out
         if n_out < 0:
             raise ValueError("more forced tokens than steps")
+        per_row = torch.is_tensor(start_pos) and start_pos.dim() > 0
+        if per_row:
+            if tuple(start_pos.shape) != (B,):
+                raise ValueError(f"per-row start_pos must have shape ({B},), got {tuple(start_pos.shape)}")
+            starts = start_pos.detach().to("cpu", torch.int64)
+            if int(starts.min()) < 0:
+                raise ValueError("negative start position")
+            last = int(starts.max())
+        else:
+            last = start_pos = int(start_pos)
         for i in mha_ip.key_value_memory_dict:
-            if start_pos + n_steps > mha_ip.key_value_memory_dict[i].shape[1]:
-                raise _lib.EvoError(f"sequence length {start_pos + n_steps} exceeds the KV cache ({mha_ip.key_value_memory_dict[i].shape[1]}) (mha.py:367)")
+            if last + n_steps > mha_ip.key_value_memory_dict[i].shape[1]:
+                raise _lib.EvoError(f"sequence length {last + n_steps} exceeds the KV cache ({mha_ip.key_value_memory_dict[i].shape[1]}) (mha.py:367)")
         with torch.cuda.device(dev), torch.no_grad():
             self._ensure_packed()
             for i in list(hy_ip.state_dict):
@@ -701,12 +764,13 @@ class StripedHyena(nn.Module):
             lp = _lib.LoopParams(forced=forced_c.data_ptr() if n_forced else None, n_forced=n_forced, forced_stride=n_forced,
                                  picked=picked.data_ptr(), picked_stride=picked.shape[1], kept_logits=kept.data_ptr(), n_out=n_out,
                                  top_k=int(top_k), top_p=float(top_p), temperature=float(temperature), seed=seed, step0=0)
-            key = ("loop", B, tuple(hy_ip.state_dict[i].data_ptr() for i in sorted(hy_ip.state_dict)),
+            key = ("loop_rows" if per_row else "loop", B, tuple(hy_ip.state_dict[i].data_ptr() for i in sorted(hy_ip.state_dict)),
                    tuple(hy_ip.fir_state_dict[i].data_ptr() for i in sorted(hy_ip.fir_state_dict)),
                    tuple((mha_ip.key_value_memory_dict[i].data_ptr(), mha_ip.key_value_memory_dict[i].shape[1]) for i in sorted(mha_ip.key_value_memory_dict)))
             st = self._loop
             if st is None or st["key"] != key:
-                st = {"key": key, "graph": None, "x": torch.empty(B, 1, dtype=torch.long, device=dev), "pos": torch.zeros(1, dtype=torch.int64, device=dev),
+                st = {"key": key, "graph": None, "x": torch.empty(B, 1, dtype=torch.long, device=dev),
+                      "pos": torch.zeros(B if per_row else 1, dtype=torch.int64, device=dev),
                       "step": torch.zeros(1, dtype=torch.int64, device=dev), "lp": torch.zeros(C.sizeof(_lib.LoopParams), dtype=torch.uint8, device=dev),
                       "lp_host": torch.zeros(C.sizeof(_lib.LoopParams), dtype=torch.uint8).pin_memory()}
                 self._loop = st
@@ -716,16 +780,23 @@ class StripedHyena(nn.Module):
             st["lp"].copy_(st["lp_host"], non_blocking=True)
             st["lp_copied"] = torch.cuda.Event()
             st["lp_copied"].record()
-            st["pos"].fill_(int(start_pos))
+            if per_row:
+                st["pos"].copy_(starts)
+            else:
+                st["pos"].fill_(int(start_pos))
             st["step"].zero_()
             st["x"].copy_(x.to(torch.long))
 
             def one_step():
-                logits = self._decode_body(st["x"], st["pos"], ipd, B)
+                logits = self._decode_body(st["x"], st["pos"], ipd, B, per_row)
                 prev = lib.evo_set_pdl(int(self.decode_pdl))
                 try:
                     check(lib.evo_sample_step(ptr(logits), ptr(st["x"]), B, V, ptr(st["lp"]), ptr(st["step"]), self._stream()), "evo_sample_step")
-                    check(lib.evo_advance_counters(ptr(st["pos"]), ptr(st["step"]), 1, self._stream()), "evo_advance_counters")
+                    if per_row:
+                        check(lib.evo_advance_positions(ptr(st["pos"]), B, 1, self._stream()), "evo_advance_positions")
+                        check(lib.evo_advance_counters(None, ptr(st["step"]), 1, self._stream()), "evo_advance_counters")
+                    else:
+                        check(lib.evo_advance_counters(ptr(st["pos"]), ptr(st["step"]), 1, self._stream()), "evo_advance_counters")
                 finally:
                     lib.evo_set_pdl(prev)
 
@@ -747,7 +818,11 @@ class StripedHyena(nn.Module):
                     lib.evo_note_graph_replay(st["launches"])
                 else:
                     one_step()
-            end = int(start_pos) + n_steps - 1          # the position the last step ran at (what the per-token protocol leaves)
+            if per_row:
+                mha_ip.lengths_per_sample = (starts + n_steps - 1).to(dev)
+                end = last + n_steps - 1
+            else:
+                end = int(start_pos) + n_steps - 1          # the position the last step ran at (what the per-token protocol leaves)
             mha_ip.seqlen_offset = hy_ip.seqlen_offset = end
             # the captured graph and its buffers stay alive in self._loop; the outputs are this call's own tensors
             return picked[:, :n_out], kept[:, :n_out]

@@ -206,7 +206,10 @@ int evo_kv_append(const void* qkv, void* cache, int B, int64_t L, int H, int hd,
  * evo_decode_qkv_prep: rotary on q,k of qkv (B, 3, H, 128) at position *pos and append of k,v at cache row *pos
  *   (flash_attn_with_kvcache's rotary + cache-append half, mha.py:502-540).
  * evo_decode_attn: one query per sequence over cache keys [0, *pos] (the attention half); split-K over nsplit.
- * evo_advance_position: *pos += delta on the stream. */
+ * evo_advance_position: *pos += delta on the stream.
+ * Per-row positions (a batch of prompts of different lengths): the _rows forms take pos as a (B) int64 DEVICE array and
+ *   use pos[b] for row b -- rotary at pos[b], k,v appended at cache row pos[b], row b attends keys [0, pos[b]].  With every
+ *   pos[b] equal they give the scalar forms' bits.  evo_advance_positions: pos[b] += delta for b < B. */
 int evo_gelu_gate_interleaved(const void* t, void* out, int64_t M, int ipad, void* stream);
 int evo_decode_qkv_prep(void* qkv, void* cache, const void* cos, const void* sin, const int64_t* pos,
                         int B, int H, int hd, int64_t max_seqlen, void* stream);
@@ -214,6 +217,11 @@ size_t evo_decode_attn_workspace(int B, int H, int nsplit);
 int evo_decode_attn(const void* qkv, const void* cache, void* out, const int64_t* pos, int B, int H, int hd,
                     int64_t max_seqlen, int nsplit, float softmax_scale, void* workspace, size_t workspace_bytes, void* stream);
 int evo_advance_position(int64_t* pos, int64_t delta, void* stream);
+int evo_decode_qkv_prep_rows(void* qkv, void* cache, const void* cos, const void* sin, const int64_t* pos,
+                             int B, int H, int hd, int64_t max_seqlen, void* stream);
+int evo_decode_attn_rows(const void* qkv, const void* cache, void* out, const int64_t* pos, int B, int H, int hd,
+                         int64_t max_seqlen, int nsplit, float softmax_scale, void* workspace, size_t workspace_bytes, void* stream);
+int evo_advance_positions(int64_t* pos, int B, int64_t delta, void* stream);
 
 /* ---- device-side sampler and generation loop: stripedhyena.sample.sample (evo/generation.py:162-167) and the host half
  * of the token loop (evo/generation.py:131-189) ----

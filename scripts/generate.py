@@ -10,7 +10,9 @@ Usage: python -m scripts.generate \
 
 Generates sequences from a prompt with the reference's sampling arguments (scripts/generate.py of evo-design/evo), on the
 evo_b200 engine.  With --cached-generation (the default) the token loop runs on the GPU (one CUDA graph per token, device
-sampler); --seed makes a sampled run reproducible.  The boolean flags keep the reference's `type=bool` parsing (any non-empty
+sampler); --seed makes a sampled run reproducible.  --prompts-csv reads the prompts from the first column of a CSV with a
+header row (semantic_design's format) and generates them all in batches of up to --batch-size, whatever their lengths
+(ragged generation: the whole prompt is prefilled, one position per row while decoding); outputs come in file order.  The boolean flags keep the reference's `type=bool` parsing (any non-empty
 value is True).
 """
 import argparse
@@ -18,6 +20,7 @@ import argparse
 import torch
 
 from evo_b200 import Evo, generate
+from evo_b200.frontend import read_prompts_csv
 
 
 def build_parser():
@@ -37,6 +40,9 @@ def build_parser():
     parser.add_argument('--seed', type=int, default=None, help='torch.manual_seed before sampling')
     parser.add_argument('--random-init', action='store_true', help='Skip the checkpoint download (random weights; smoke runs offline)')
     parser.add_argument('--model-dir', type=str, default=None, help='Directory of an already downloaded HF snapshot')
+    parser.add_argument('--prompts-csv', type=str, default=None,
+                        help='CSV whose first column (after a header row) holds the prompts; generates every prompt once, batched whatever their lengths')
+    parser.add_argument('--batch-size', type=int, default=64, help='Prompts per decode batch with --prompts-csv')
     return parser
 
 
@@ -48,6 +54,10 @@ def main(argv=None):
     if args.seed is not None:
         torch.manual_seed(args.seed)
     print('Generated sequences:')
+    if args.prompts_csv is not None:
+        return generate(read_prompts_csv(args.prompts_csv), model, tokenizer, n_tokens=args.n_tokens, temperature=args.temperature,
+                        top_k=args.top_k, top_p=args.top_p, cached_generation=True, prepend_bos=args.prepend_bos, device=args.device,
+                        verbose=args.verbose, ragged=True, batch_size=args.batch_size)
     return generate([args.prompt] * args.n_samples, model, tokenizer, n_tokens=args.n_tokens, temperature=args.temperature,
                     top_k=args.top_k, top_p=args.top_p, cached_generation=args.cached_generation, batched=args.batched,
                     prepend_bos=args.prepend_bos, device=args.device, verbose=args.verbose)
