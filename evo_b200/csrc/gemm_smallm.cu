@@ -100,7 +100,8 @@ template <int EPI> struct RowGroups { static constexpr int R = EPI == EVO_EPI_GE
 
 // One decode step of the Hyena operator for channel `ch` of head `tile`, 16 batch rows: the arithmetic of hyena_step_kernel
 // (hyena.cu; engine.step_fir + step_iir of the reference) on the in-projection's fp32 sums z2/z1/zv (x2, x1, v rows of the head).
-// Every rounding point is the one the two-kernel path has: z = bf16(sum + bias) is what EVO_EPI_BIAS would have stored.
+// Every rounding point is the one the two-kernel path has: z = bf16(sum + bias), as EVO_EPI_BIAS stores it.  The fp32 sum itself
+// equals that launch's only where both cut the K range at the same k-blocks (the tile count, and so the stream-K split, differs).
 __device__ __forceinline__ void hyena_step16(const SmArgs& g, int tile, int row, int b0, const float (&z2)[16], const float (&z1)[16], const float (&zv)[16]) {
   const int D = g.D, ch = tile * WROWS + row;
   const long long C3 = 3LL * D;

@@ -352,7 +352,8 @@ extern "C" int evo_hyena_fwd(const evo_hyena_params* p, void* workspace, size_t 
     if ((rc = ensure_dyn_smem(hyena_scan_tma_kernel<true>, smem_bytes(STAGES), done_s))) return rc;
     if ((rc = ensure_dyn_smem(hyena_scan_tma_kernel<false>, smem_bytes(STAGES), done_o))) return rc;
     // 1 (default) = mode-split kernel (hyena_ms.cuh: 8 compute warps, 4 modal states per thread); 0 = round-1 kernel
-    // (4 compute warps, 8 states per thread), kept for A/B timing and as a second implementation in the parity tests
+    // (4 compute warps, 8 states per thread), kept for A/B timing and as a second implementation that
+    // tests/test_gpu_hyena_paths.py holds to the same oracle bars and compares with this one
     const char* env_v = getenv("EVO_B200_HYENA_VARIANT");      // read per call: experiments flip it inside one process
     const int variant = env_v ? atoi(env_v) : 1;
     static unsigned long long done_ms = 0, done_mo = 0;

@@ -217,8 +217,9 @@ class StripedHyena(nn.Module):
         self.decode_streamk = os.environ.get("EVO_B200_DECODE_STREAMK", "1") != "0"
         # programmatic dependent launch inside a decode step (evo_set_pdl): 0 off, 1 every kernel, 2 weight-streaming GEMMs only
         self.decode_pdl = int(os.environ.get("EVO_B200_DECODE_PDL", "4"))
-        # the Hyena decode step inside the in-projection GEMM's epilogue (EVO_EPI_HYENA_STEP).  Bit-identical to the separate
-        # evo_hyena_step launch, but the step of a tile runs on the 128 epilogue threads of its last contributor -- 16 batch rows x 8 states of dependent
+        # the Hyena decode step inside the in-projection GEMM's epilogue (EVO_EPI_HYENA_STEP).  The step arithmetic is bit-identical
+        # to the separate evo_hyena_step launch; z matches EVO_EPI_BIAS up to the stream-K split of the K sum, which depends on the tile
+        # height (DESIGN.md).  The step of a tile runs on the 128 epilogue threads of its last contributor -- 16 batch rows x 8 states of dependent
         # load -> update -> store per thread in the GEMM's serial tail -- where the stand-alone kernel spreads the same 8 MB of state
         # traffic over 524 288 threads.  Off by default; kept as a tested option.
         self.decode_fused_step = os.environ.get("EVO_B200_DECODE_FUSED_STEP", "0") != "0"
