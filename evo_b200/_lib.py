@@ -44,6 +44,21 @@ class HyenaParams(C.Structure):
                 ("force_segments", C.c_int), ("state_only", C.c_int), ("reuse_segment_states", C.c_int)]
 
 
+class HyenaVarlenParams(C.Structure):
+    _fields_ = [("z", C.c_void_p), ("y", C.c_void_p), ("fir_w", C.c_void_p), ("fir_b", C.c_void_p), ("Dskip", C.c_void_p),
+                ("poles", C.c_void_p), ("residues", C.c_void_p),
+                ("cu_seqlens", C.c_void_p), ("n_seq", C.c_int), ("T", C.c_int64), ("max_seqlen", C.c_int64),
+                ("D", C.c_int), ("S", C.c_int), ("nheads", C.c_int),
+                ("state_out", C.c_void_p), ("fir_state_out", C.c_void_p), ("seg_len", C.c_int64)]
+
+
+class AttnVarlenParams(C.Structure):
+    _fields_ = [("q", C.c_void_p), ("k", C.c_void_p), ("v", C.c_void_p), ("out", C.c_void_p),
+                ("q_tok_stride", C.c_int64), ("kv_tok_stride", C.c_int64),
+                ("cu_seqlens", C.c_void_p), ("n_seq", C.c_int), ("T", C.c_int64), ("max_seqlen", C.c_int64),
+                ("H", C.c_int), ("hd", C.c_int), ("softmax_scale", C.c_float)]
+
+
 class AttnParams(C.Structure):
     _fields_ = [("q", C.c_void_p), ("k", C.c_void_p), ("v", C.c_void_p), ("out", C.c_void_p),
                 ("q_tok_stride", C.c_int64), ("kv_tok_stride", C.c_int64),
@@ -81,6 +96,8 @@ SIGNATURES = {
     "evo_set_pdl": (C.c_int, [C.c_int]),
     "evo_hyena_fwd_workspace": (C.c_size_t, [C.POINTER(HyenaParams)]),
     "evo_hyena_fwd": (C.c_int, [C.POINTER(HyenaParams), C.c_void_p, C.c_size_t, C.c_void_p]),
+    "evo_hyena_fwd_varlen_workspace": (C.c_size_t, [C.POINTER(HyenaVarlenParams)]),
+    "evo_hyena_fwd_varlen": (C.c_int, [C.POINTER(HyenaVarlenParams), C.c_void_p, C.c_size_t, C.c_void_p]),
     "evo_hyena_step": (C.c_int, [C.c_void_p] * 9 + [C.c_int] * 4 + [C.c_void_p]),
     "evo_hyena_combine_states": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "evo_peer_publish": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
@@ -90,6 +107,8 @@ SIGNATURES = {
     "evo_attn_fwd_workspace": (C.c_size_t, [C.POINTER(AttnParams), C.c_int]),
     "evo_attn_fwd_ws": (C.c_int, [C.POINTER(AttnParams), C.c_int, C.c_void_p, C.c_size_t, C.c_void_p]),
     "evo_kv_append": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_int64, C.c_int64, C.c_void_p]),
+    "evo_attn_fwd_varlen": (C.c_int, [C.POINTER(AttnVarlenParams), C.c_void_p]),
+    "evo_kv_append_varlen": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_int64, C.c_int, C.c_int, C.c_int64, C.c_void_p]),
     "evo_gelu_gate_interleaved": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p]),
     "evo_decode_qkv_prep": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int64, C.c_void_p]),
     "evo_decode_attn_workspace": (C.c_size_t, [C.c_int, C.c_int, C.c_int]),

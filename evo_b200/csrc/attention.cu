@@ -15,6 +15,7 @@
 // PV product, fp32 accumulation, single bf16 rounding of the output.
 #include "common.cuh"
 #include "wgmma.cuh"
+#include <type_traits>
 #include "../../include/evo_b200.h"
 
 using namespace evo;
@@ -39,12 +40,20 @@ struct AttArgs {
   long long Lq, Lk, q_pos0;
   float scale_log2;              // softmax_scale * log2(e)
 };
+struct AttArgsV : AttArgs {      // packed sequences (VARLEN); AttArgs itself stays as it is, and so does its kernel
+  const long long* cu_seqlens;   // (B + 1) row offsets; Lq = Lk = the longest length
+  long long T;                   // packed rows
+};
 
 __device__ __forceinline__ float ex2(float x) { float y; asm volatile("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 
+// VARLEN: grid row b is packed sequence b = rows [cu[b], cu[b+1]) of (HD, H, T, 1) maps.  Query and key tiles start at the
+// sequence's first row, exactly as in a batch-1 call on it; keys past its end are hidden by the causal mask and query rows past
+// its end are not stored, so the output is that call's bits.
+template <bool VARLEN>
 __global__ void __launch_bounds__(ATT_THREADS, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                const __grid_constant__ CUtensorMap tmV, const AttArgs a) {
+                const __grid_constant__ CUtensorMap tmV, const std::conditional_t<VARLEN, AttArgsV, AttArgs> a) {
   extern __shared__ __align__(1024) uint8_t smem[];            // 128B-swizzled tiles need 1024-byte alignment
   if ((smem_u32(smem) & 1023u) != 0) __trap();               // fail loudly, never compute on a misaligned tile
   uint8_t* sQ = smem;
@@ -58,12 +67,19 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   uint64_t* v_empty = v_full + KV_STAGES;
 
   const int wg = threadIdx.x >> 7, tid = threadIdx.x & 127;
-  const int n_qblk = (int)((a.Lq + BQ - 1) / BQ);
-  const int qblk = n_qblk - 1 - (int)blockIdx.x;      // longest (latest) blocks first
   const int h = blockIdx.y, b = blockIdx.z;
+  long long Lq = a.Lq, Lk = a.Lk, row0 = 0;
+  if constexpr (VARLEN) {          // clamped, so that a malformed cu_seqlens cannot move a load or store outside [0, T)
+    row0 = min(max(a.cu_seqlens[b], 0LL), a.T);
+    Lq = Lk = min(min(a.cu_seqlens[b + 1], a.T) - row0, a.Lq);
+  }
+  const int n_qblk = (int)((Lq + BQ - 1) / BQ);
+  const int qblk = n_qblk - 1 - (int)blockIdx.x;      // longest (latest) blocks first
+  if (VARLEN && qblk < 0) return;                     // past this sequence's last query block
+  const int zb = VARLEN ? 0 : b;
   const long long q0 = (long long)qblk * BQ;
   // keys visible to this block: j <= q_pos0 + q0 + 127, j < Lk
-  const long long last_key = min(a.Lk - 1, a.q_pos0 + q0 + BQ - 1);
+  const long long last_key = min(Lk - 1, a.q_pos0 + q0 + BQ - 1);
   const int n_kv = (int)(last_key / BKV) + 1;
 
   if (threadIdx.x == 0) {
@@ -79,20 +95,20 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     setmaxnreg_dec<40>();
     if (tid == 0) {
       mbar_arrive_expect_tx(q_full, TILE_BYTES);
-      tma_load_4d(sQ, &tmQ, q_full, 0, h, (int)q0, b);
-      tma_load_4d(sQ + HALF_BYTES, &tmQ, q_full, 64, h, (int)q0, b);
+      tma_load_4d(sQ, &tmQ, q_full, 0, h, (int)(row0 + q0), zb);
+      tma_load_4d(sQ + HALF_BYTES, &tmQ, q_full, 64, h, (int)(row0 + q0), zb);
       for (int j = 0; j < n_kv; ++j) {
         const int st = j % KV_STAGES;
         const uint32_t ph = (uint32_t)(j / KV_STAGES) & 1;
-        const int key0 = j * BKV;
+        const int key0 = (int)row0 + j * BKV;
         mbar_wait(&k_empty[st], ph ^ 1);
         mbar_arrive_expect_tx(&k_full[st], TILE_BYTES);
-        tma_load_4d(sK + st * TILE_BYTES, &tmK, &k_full[st], 0, h, key0, b);
-        tma_load_4d(sK + st * TILE_BYTES + HALF_BYTES, &tmK, &k_full[st], 64, h, key0, b);
+        tma_load_4d(sK + st * TILE_BYTES, &tmK, &k_full[st], 0, h, key0, zb);
+        tma_load_4d(sK + st * TILE_BYTES + HALF_BYTES, &tmK, &k_full[st], 64, h, key0, zb);
         mbar_wait(&v_empty[st], ph ^ 1);       // (d, H, key, B): two d-halves of 128 keys x 64 d
         mbar_arrive_expect_tx(&v_full[st], TILE_BYTES);
-        tma_load_4d(sV + st * TILE_BYTES, &tmV, &v_full[st], 0, h, key0, b);
-        tma_load_4d(sV + st * TILE_BYTES + HALF_BYTES, &tmV, &v_full[st], 64, h, key0, b);
+        tma_load_4d(sV + st * TILE_BYTES, &tmV, &v_full[st], 0, h, key0, zb);
+        tma_load_4d(sV + st * TILE_BYTES + HALF_BYTES, &tmV, &v_full[st], 64, h, key0, zb);
       }
     }
   } else {
@@ -179,8 +195,8 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
       lt += __shfl_xor_sync(0xffffffffu, lt, 2);
       const float inv_l = 1.f / lt;
       const long long tok = q0 + r0 + 8 * hr;
-      if (tok >= a.Lq) continue;
-      bf16* orow = a.out + (((long long)b * a.Lq + tok) * a.H + h) * HD;
+      if (tok >= Lq) continue;
+      bf16* orow = a.out + (((VARLEN ? row0 : (long long)b * a.Lq) + tok) * a.H + h) * HD;
       if (a.n_out_peers > 0) {
         const long long pr = tok / a.out_rows_per_peer;
         orow = a.out_peer[pr < a.n_out_peers ? pr : 0] + (tok - pr * a.out_rows_per_peer) * a.out_row_stride + a.out_col0 + (long long)h * HD;
@@ -266,7 +282,40 @@ extern "C" int evo_attn_fwd_ws(const evo_attn_params* p, int variant, void* work
   for (int i = 0; i < 8; ++i) a.out_peer[i] = i < p->n_out_peers ? (bf16*)p->out_peers[i] : nullptr;
   dim3 grid((unsigned)((p->Lq + BQ - 1) / BQ), p->H, p->B);
   static unsigned long long done = 0;
-  if ((rc = ensure_dyn_smem(attn_fwd_kernel, ATT_SMEM, done))) return rc;
-  attn_fwd_kernel<<<grid, ATT_THREADS, ATT_SMEM, st>>>(tmQ, tmK, tmV, a);
+  if ((rc = ensure_dyn_smem(attn_fwd_kernel<false>, ATT_SMEM, done))) return rc;
+  attn_fwd_kernel<false><<<grid, ATT_THREADS, ATT_SMEM, st>>>(tmQ, tmK, tmV, a);
   return check_launch("evo_attn_fwd");
+}
+
+extern "C" int evo_attn_fwd_varlen(const evo_attn_varlen_params* p, void* stream) {
+  EVO_REQUIRE(p->hd == HD, "evo_attn_fwd_varlen: head_dim %d unsupported (kernel is specialised for 128)", p->hd);
+  EVO_REQUIRE(p->q_tok_stride % 8 == 0 && p->kv_tok_stride % 8 == 0, "evo_attn_fwd_varlen: strides must be multiples of 8 elements");
+  EVO_REQUIRE(p->n_seq > 0 && p->n_seq <= 65535 && p->H > 0 && p->H <= 65535, "evo_attn_fwd_varlen: bad sequence count %d or head count %d", p->n_seq, p->H);
+  EVO_REQUIRE(p->cu_seqlens != nullptr && p->max_seqlen > 0 && p->max_seqlen <= p->T && p->T < (1LL << 31),
+              "evo_attn_fwd_varlen: needs cu_seqlens and 0 < max_seqlen <= T < 2^31 (max_seqlen %lld, T %lld)", (long long)p->max_seqlen, (long long)p->T);
+  cudaStream_t st = (cudaStream_t)stream;
+  CUtensorMap tmQ, tmK, tmV;
+  int rc;
+  {
+    uint64_t dims[4] = {(uint64_t)HD, (uint64_t)p->H, (uint64_t)p->T, 1};
+    uint64_t str[3] = {(uint64_t)HD * 2, (uint64_t)p->q_tok_stride * 2, (uint64_t)p->T * p->q_tok_stride * 2};
+    uint32_t box[4] = {64, 1, BQ, 1};
+    if ((rc = make_tmap_4d(&tmQ, p->q, dims, str, box))) return rc;
+  }
+  {
+    uint64_t dims[4] = {(uint64_t)HD, (uint64_t)p->H, (uint64_t)p->T, 1};
+    uint64_t str[3] = {(uint64_t)HD * 2, (uint64_t)p->kv_tok_stride * 2, (uint64_t)p->T * p->kv_tok_stride * 2};
+    uint32_t box[4] = {64, 1, BKV, 1};
+    if ((rc = make_tmap_4d(&tmK, p->k, dims, str, box))) return rc;
+    if ((rc = make_tmap_4d(&tmV, p->v, dims, str, box))) return rc;
+  }
+  AttArgsV a = {};
+  a.out = (bf16*)p->out; a.B = p->n_seq; a.H = p->H; a.Lq = a.Lk = p->max_seqlen; a.q_pos0 = 0;
+  a.scale_log2 = p->softmax_scale * 1.4426950408889634f;
+  a.cu_seqlens = (const long long*)p->cu_seqlens; a.T = p->T;
+  dim3 grid((unsigned)((p->max_seqlen + BQ - 1) / BQ), p->H, p->n_seq);
+  static unsigned long long done = 0;
+  if ((rc = ensure_dyn_smem(attn_fwd_kernel<true>, ATT_SMEM, done))) return rc;
+  attn_fwd_kernel<true><<<grid, ATT_THREADS, ATT_SMEM, st>>>(tmQ, tmK, tmV, a);
+  return check_launch("evo_attn_fwd_varlen");
 }

@@ -242,6 +242,31 @@ extern "C" int evo_kv_append(const void* qkv, void* cache, int B, int64_t L, int
   return check_launch("evo_kv_append");
 }
 
+// packed sequences: grid row b copies sequence b's rows [cu[b], cu[b+1]) to cache rows [0, len) of batch row b
+__global__ void kv_append_varlen_kernel(const uint4* __restrict__ qkv, uint4* __restrict__ cache, const long long* __restrict__ cu,
+                                        long long T, long long max_len, int row_vec, int64_t cache_len) {
+  const int b = blockIdx.y;
+  const long long row0 = min(max(cu[b], 0LL), T);
+  const long long len = min(min(cu[b + 1], T) - row0, max_len);
+  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const int c = (int)(idx % (2 * row_vec));
+  const int64_t l = idx / (2 * row_vec);
+  if (l >= len) return;
+  cache[((int64_t)b * cache_len + l) * (2 * row_vec) + c] = qkv[(row0 + l) * (3 * row_vec) + row_vec + c];
+}
+
+extern "C" int evo_kv_append_varlen(const void* qkv, void* cache, const int64_t* cu_seqlens, int n_seq, int64_t T, int64_t max_seqlen,
+                                    int H, int hd, int64_t cache_len, void* stream) {
+  EVO_REQUIRE(n_seq > 0 && n_seq <= 65535 && cu_seqlens != nullptr, "evo_kv_append_varlen: bad sequence count %d or no cu_seqlens", n_seq);
+  EVO_REQUIRE(max_seqlen > 0 && max_seqlen <= T && max_seqlen <= cache_len,
+              "evo_kv_append_varlen: longest sequence %lld must be in (0, min(T %lld, cache %lld)]", (long long)max_seqlen, (long long)T, (long long)cache_len);
+  EVO_REQUIRE((H * hd) % 8 == 0, "evo_kv_append_varlen: H * hd must be a multiple of 8");
+  const int row_vec = H * hd / 8;
+  const int64_t per_seq = max_seqlen * 2 * row_vec;
+  kv_append_varlen_kernel<<<dim3((unsigned)((per_seq + 255) / 256), n_seq), 256, 0, (cudaStream_t)stream>>>(
+      (const uint4*)qkv, (uint4*)cache, (const long long*)cu_seqlens, T, max_seqlen, row_vec, cache_len);
+  return check_launch("evo_kv_append_varlen");
+}
 
 // ------------------------------------------------------------------ scoring epilogue
 // out[r] = log_softmax(logits[r, :])[target[r]], fp32 statistics; one warp per row.

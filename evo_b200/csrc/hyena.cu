@@ -226,6 +226,21 @@ __global__ void fir_state_kernel(const bf16* __restrict__ z, const bf16* __restr
   }
 }
 
+// packed sequences: sequence b's last two z rows, zero history before its first row
+__global__ void fir_state_varlen_kernel(const bf16* __restrict__ z, const long long* __restrict__ cu, bf16* __restrict__ out,
+                                        int n_seq, long long T, long long max_len, long long C3) {
+  long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;   // (b, c)
+  if (idx >= (long long)n_seq * C3) return;
+  long long b = idx / C3, c = idx % C3;
+  const long long row0 = min(max(cu[b], 0LL), T);
+  const long long len = min(min(cu[b + 1], T) - row0, max_len);
+#pragma unroll
+  for (int k = 0; k < 2; ++k) {
+    long long t = len - 2 + k;
+    out[idx * 2 + k] = t >= 0 ? z[(row0 + t) * C3 + c] : __float2bfloat16_rn(0.f);
+  }
+}
+
 // decode step (engine.step_fir + step_iir): 8 lanes per (b, channel).  Lane s owns modal state s (its pole, residue
 // and state are one coalesced 8-byte load each); lanes 0..2 run the three FIR channels (x2, x1, v); lane 0 folds the
 // eight residue products in the reference's order (sequential fma chain) and writes y.
@@ -410,6 +425,77 @@ extern "C" int evo_hyena_fwd(const evo_hyena_params* p, void* workspace, size_t 
     long long n = (long long)p->B * 3 * p->D;
     fir_state_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>((const bf16*)p->z, (const bf16*)p->halo, (bf16*)p->fir_state_out, p->B, p->L, 3LL * p->D);
     if ((rc = check_launch("fir_state"))) return rc;
+  }
+  return 0;
+}
+
+// packed sequences: nseg = pick_segments(B = n_seq, L = max_seqlen) and one common seg_len -- on equal lengths exactly the
+// geometry evo_hyena_fwd gives the (n_seq, L) batch, so the two compute the same bits
+static int varlen_geometry(const evo_hyena_varlen_params* p, int& nseg, long long& seg_len) {
+  EVO_REQUIRE(p->S == NS, "evo_hyena_fwd_varlen: state_size %d unsupported (kernel is specialised for %d)", p->S, NS);
+  EVO_REQUIRE(p->nheads > 0 && p->D % p->nheads == 0 && p->D / p->nheads == 128 && p->D % evo_hy2::CH_PER_CTA == 0,
+              "evo_hyena_fwd_varlen: needs head_dim 128 and D %% 256 == 0 (D %d, %d heads)", p->D, p->nheads);
+  EVO_REQUIRE(p->n_seq > 0 && p->n_seq <= 65535, "evo_hyena_fwd_varlen: bad sequence count %d", p->n_seq);
+  EVO_REQUIRE(p->cu_seqlens != nullptr && p->max_seqlen > 0 && p->max_seqlen <= p->T && p->T < (1LL << 31),
+              "evo_hyena_fwd_varlen: needs cu_seqlens and 0 < max_seqlen <= T < 2^31 (max_seqlen %lld, T %lld)", (long long)p->max_seqlen, (long long)p->T);
+  EVO_REQUIRE(p->seg_len >= 0, "evo_hyena_fwd_varlen: negative seg_len");
+  if (p->seg_len > 0) {
+    seg_len = p->seg_len;
+  } else {
+    evo_hyena_params q = {};
+    q.B = p->n_seq; q.L = p->max_seqlen; q.D = p->D; q.nheads = p->nheads;
+    const int n = pick_segments(&q);
+    seg_len = (q.L + n - 1) / n;
+  }
+  nseg = (int)((p->max_seqlen + seg_len - 1) / seg_len);
+  EVO_REQUIRE(nseg <= 65535, "evo_hyena_fwd_varlen: %d segments", nseg);
+  return 0;
+}
+
+extern "C" size_t evo_hyena_fwd_varlen_workspace(const evo_hyena_varlen_params* p) {
+  int nseg; long long seg_len;
+  if (varlen_geometry(p, nseg, seg_len) || nseg <= 1) return 0;
+  return (size_t)p->n_seq * nseg * p->D * NS * 2 * sizeof(float);
+}
+
+extern "C" int evo_hyena_fwd_varlen(const evo_hyena_varlen_params* p, void* workspace, size_t workspace_bytes, void* stream) {
+  int nseg; long long seg_len;
+  int rc;
+  if ((rc = varlen_geometry(p, nseg, seg_len))) return rc;
+  EVO_REQUIRE(p->z != nullptr && p->y != nullptr, "evo_hyena_fwd_varlen: z or y is NULL");
+  const size_t need = evo_hyena_fwd_varlen_workspace(p);
+  EVO_REQUIRE(workspace_bytes >= need && (need == 0 || workspace), "evo_hyena_fwd_varlen: workspace too small (%zu < %zu)", workspace_bytes, need);
+  cudaStream_t st = (cudaStream_t)stream;
+  using namespace evo_hy2;
+  CUtensorMap tmZ;
+  uint64_t dims[3] = {(uint64_t)3 * p->D, (uint64_t)p->T, 1};
+  uint64_t str[2] = {(uint64_t)3 * p->D * 2, (uint64_t)p->T * 3 * p->D * 2};
+  uint32_t box[3] = {128, (uint32_t)T2, 1};
+  if ((rc = make_tmap_nd_bf16(&tmZ, p->z, 3, dims, str, box, false))) return rc;
+  evo_hy3::Args2V a = {};
+  a.y = (bf16*)p->y; a.z = (const bf16*)p->z;
+  a.fir_w = (const bf16*)p->fir_w; a.fir_b = (const bf16*)p->fir_b; a.Dskip = (const bf16*)p->Dskip;
+  a.poles = p->poles; a.residues = p->residues; a.state_out = p->state_out;
+  a.seg_states = (float*)workspace; a.B = p->n_seq; a.D = p->D; a.nseg = nseg; a.L = p->max_seqlen; a.seg_len = seg_len;
+  a.cu_seqlens = (const long long*)p->cu_seqlens; a.T = p->T;
+  a.nst = 4;
+  static unsigned long long done_s = 0, done_o = 0;
+  if ((rc = ensure_dyn_smem(evo_hy3::hyena_scan_ms_kernel<true, true>, smem_bytes(STAGES), done_s))) return rc;
+  if ((rc = ensure_dyn_smem(evo_hy3::hyena_scan_ms_kernel<false, true>, smem_bytes(STAGES), done_o))) return rc;
+  const int SMEM_BYTES = smem_bytes(a.nst);
+  dim3 grid(p->D / CH_PER_CTA, p->n_seq, nseg), block(evo_hy3::THREADS);
+  if (nseg > 1) {
+    dim3 g2(grid.x, grid.y, nseg - 1);
+    evo_hy3::hyena_scan_ms_kernel<true, true><<<g2, block, SMEM_BYTES, st>>>(tmZ, a);
+    if ((rc = check_launch("hyena_scan_varlen<state>"))) return rc;
+  }
+  evo_hy3::hyena_scan_ms_kernel<false, true><<<grid, block, SMEM_BYTES, st>>>(tmZ, a);
+  if ((rc = check_launch("hyena_scan_varlen<out>"))) return rc;
+  if (p->fir_state_out) {
+    long long n = (long long)p->n_seq * 3 * p->D;
+    fir_state_varlen_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>((const bf16*)p->z, (const long long*)p->cu_seqlens, (bf16*)p->fir_state_out,
+                                                                         p->n_seq, p->T, p->max_seqlen, 3LL * p->D);
+    if ((rc = check_launch("fir_state_varlen"))) return rc;
   }
   return 0;
 }

@@ -17,6 +17,7 @@
 // fma-pipe instructions per token per channel pair: 68 (was 67); ALU conversions ~21 (was ~38).
 #pragma once
 #include "hyena_tma.cuh"
+#include <type_traits>
 
 namespace evo_hy3 {
 
@@ -40,13 +41,21 @@ constexpr int THREADS = (CWARPS + 1) * 32;   // + 1 TMA producer warp
 constexpr int G = 8;                         // tokens per group
 constexpr int smem_bytes(int nst) { return evo_hy2::smem_bytes(nst); }
 
+struct Args2V : Args2 {                      // packed sequences (VARLEN); Args2 itself stays as it is, and so do its kernels
+  const long long* cu_seqlens;               // (B + 1) row offsets; Args2::L is the longest length
+  long long T;                               // packed rows
+};
+
 __device__ __forceinline__ uint32_t mul_bf2(uint32_t a, uint32_t b) { uint32_t d; asm("mul.rn.bf16x2 %0, %1, %2;" : "=r"(d) : "r"(a), "r"(b)); return d; }
 __device__ __forceinline__ uint32_t add_bf2(uint32_t a, uint32_t b) { uint32_t d; asm("add.rn.bf16x2 %0, %1, %2;" : "=r"(d) : "r"(a), "r"(b)); return d; }
 __device__ __forceinline__ uint32_t ldg32(const bf16* p) { return __ldg(reinterpret_cast<const unsigned int*>(p)); }
 
-template <bool STATE_ONLY>
+// VARLEN: packed sequences (evo_hyena_fwd_varlen).  Grid row b is sequence b = rows [cu[b], cu[b+1]) of a (3D, T, 1) tensor map;
+// a.L is the longest length.  Every segment but a sequence's last is full (one seg_len for all), so the carry below holds unchanged;
+// a tile that reaches into the next sequence goes through the ragged-tile path (n_valid), so no foreign token enters the scan.
+template <bool STATE_ONLY, bool VARLEN = false>
 __global__ void __launch_bounds__(THREADS, 1)
-hyena_scan_ms_kernel(const __grid_constant__ CUtensorMap tmZ, const Args2 a) {
+hyena_scan_ms_kernel(const __grid_constant__ CUtensorMap tmZ, const std::conditional_t<VARLEN, Args2V, Args2> a) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 127) & ~(uintptr_t)127);
   const int NST = a.nst;
@@ -56,7 +65,13 @@ hyena_scan_ms_kernel(const __grid_constant__ CUtensorMap tmZ, const Args2 a) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int cb = blockIdx.x, b = blockIdx.y, seg = blockIdx.z;
   const long long t0 = (long long)seg * a.seg_len;
-  const long long t1 = min(a.L, t0 + a.seg_len);
+  long long row0 = 0, len = a.L;
+  if constexpr (VARLEN) {          // clamped, so that a malformed cu_seqlens cannot move a load or store outside [0, T)
+    row0 = min(max(a.cu_seqlens[b], 0LL), a.T);
+    len = min(min(a.cu_seqlens[b + 1], a.T) - row0, a.L);
+    if (t0 >= len) return;
+  }
+  const long long t1 = min(len, t0 + a.seg_len);
   const int n_tiles = t1 > t0 ? (int)((t1 - t0 + T2 - 1) / T2) : 0;
 
   if (threadIdx.x == 0) {
@@ -73,19 +88,20 @@ hyena_scan_ms_kernel(const __grid_constant__ CUtensorMap tmZ, const Args2 a) {
         const int st = k % NST;
         mbar_wait(&empty[st], ((uint32_t)(k / NST) & 1) ^ 1);
         uint8_t* dst = smem + st * STAGE_BYTES;
-        const int row = (int)(t0 + (long long)k * T2);
+        const int row = (int)(row0 + t0 + (long long)k * T2);
+        const int zb3 = VARLEN ? 0 : b;
         if (STATE_ONLY) {
           mbar_arrive_expect_tx(&full[st], 4 * SUB_BYTES);
 #pragma unroll
           for (int hh = 0; hh < 2; ++hh)
 #pragma unroll
             for (int w = 1; w < 3; ++w)
-              tma_load_3d(dst + (hh * 3 + w) * SUB_BYTES, &tmZ, &full[st], cb * 768 + hh * 384 + w * 128, row, b);
+              tma_load_3d(dst + (hh * 3 + w) * SUB_BYTES, &tmZ, &full[st], cb * 768 + hh * 384 + w * 128, row, zb3);
         } else {
           mbar_arrive_expect_tx(&full[st], STAGE_BYTES);
 #pragma unroll
           for (int s6 = 0; s6 < 6; ++s6)
-            tma_load_3d(dst + s6 * SUB_BYTES, &tmZ, &full[st], cb * 768 + s6 * 128, row, b);
+            tma_load_3d(dst + s6 * SUB_BYTES, &tmZ, &full[st], cb * 768 + s6 * 128, row, zb3);
         }
       }
     }
@@ -156,7 +172,8 @@ hyena_scan_ms_kernel(const __grid_constant__ CUtensorMap tmZ, const Args2 a) {
   }
 
   // FIR history z[t0-2], z[t0-1]: fp32 pair for the owned channel, packed words for x2 (half 0 only uses them)
-  const bf16* zb = a.z + (long long)b * a.L * C3;
+  const long long seq_row = VARLEN ? row0 : (long long)b * a.L;      // z / y row of the sequence's token 0
+  const bf16* zb = a.z + seq_row * C3;
   float2 ho[2];
   uint32_t h2q[2];
 #pragma unroll
@@ -170,7 +187,7 @@ hyena_scan_ms_kernel(const __grid_constant__ CUtensorMap tmZ, const Args2 a) {
   }
 
   const long long ystride = a.D / 2;        // in 32-bit words
-  uint32_t* yrow = STATE_ONLY ? nullptr : reinterpret_cast<uint32_t*>(a.y + ((long long)b * a.L + t0) * a.D + ch) + (long long)(4 * half) * ystride;
+  uint32_t* yrow = STATE_ONLY ? nullptr : reinterpret_cast<uint32_t*>(a.y + (seq_row + t0) * a.D + ch) + (long long)(4 * half) * ystride;
 
   auto do_group = [&](uint32_t tile, int j0, int n_valid, uint32_t* ydst) {
     // ---- stage A: the owned short FIR (fp32 accumulate, rp) + bias (rp) for all G tokens
@@ -255,7 +272,7 @@ hyena_scan_ms_kernel(const __grid_constant__ CUtensorMap tmZ, const Args2 a) {
 
   float* dst = nullptr;
   if (STATE_ONLY) dst = a.seg_states + ((((long long)b * a.nseg + seg) * a.D + ch) * NS) * 2;
-  else if (a.state_out && seg == a.nseg - 1) dst = a.state_out + (((long long)b * a.D + ch) * NS) * 2;
+  else if (a.state_out && (VARLEN ? t1 == len : seg == a.nseg - 1)) dst = a.state_out + (((long long)b * a.D + ch) * NS) * 2;
   if (dst) {
     float2* e = reinterpret_cast<float2*>(dst) + m0;
 #pragma unroll

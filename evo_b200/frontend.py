@@ -105,6 +105,27 @@ def ragged_batches(lengths: Sequence[int], n_new: int, batch_size: int = 64, ali
     return out
 
 
+def packs(lengths: Sequence[int], max_tokens: int, bos: int = 1) -> List[Tuple[List[int], List[int]]]:
+    """Plan of packed forwards: [(row indices, cu_seqlens)].  Sequences are taken longest first and cut into packs of at most
+    `max_tokens` tokens, `bos` extra token per sequence included; inside a pack they stay longest first, so the longest
+    sequences' blocks launch first.  A sequence longer than `max_tokens` gets a pack of its own.  cu_seqlens is the pack's
+    n + 1 offsets in tokens (flash-attn varlen convention)."""
+    if max_tokens < 1:
+        raise ValueError("max_tokens must be >= 1")
+    order = sorted(range(len(lengths)), key=lambda i: (-lengths[i], i))
+    out, rows, cu = [], [], [0]
+    for i in order:
+        n = lengths[i] + bos
+        if rows and cu[-1] + n > max_tokens:
+            out.append((rows, cu))
+            rows, cu = [], [0]
+        rows.append(i)
+        cu.append(cu[-1] + n)
+    if rows:
+        out.append((rows, cu))
+    return out
+
+
 # ----------------------------------------------------------------------------- host bytes -> device ids
 def device_batch(seqs: Sequence[str], tokenizer: CharLevelTokenizer, prepend_bos: bool = True, device: str = "cuda:0",
                  dtype: torch.dtype = torch.long) -> Tuple[torch.Tensor, List[int]]:
@@ -137,12 +158,35 @@ def device_batch(seqs: Sequence[str], tokenizer: CharLevelTokenizer, prepend_bos
     return ids, lengths
 
 
+def packed_ids(seqs: Sequence[str], tokenizer: CharLevelTokenizer, device: str = "cuda:0") -> torch.Tensor:
+    """(T,) int64 ids on `device` of the sequences end to end, each as [BOS] + bytes: device_batch's one pinned uint8 transfer,
+    then the padding of its (n, width) matrix dropped on the device."""
+    ids, lengths = device_batch(seqs, tokenizer, prepend_bos=True, device=device)
+    keep = torch.arange(ids.shape[1], device=ids.device)[None, :] <= torch.tensor(lengths, device=ids.device)[:, None]
+    return ids[keep]
+
+
 def score_many(seqs: Sequence[str], model, tokenizer: CharLevelTokenizer, batch_size: int = 32, max_tokens: int = 1 << 17,
-               reduce_method: str = "mean", device: str = "cuda:0") -> List[float]:
+               reduce_method: str = "mean", device: str = "cuda:0", packed: bool = False) -> List[float]:
     """score_sequences over an arbitrary list in length buckets; scores come back in input order (the loop of
-    scripts/score.py:45-55 with bounded padding)."""
+    scripts/score.py:45-55 with bounded padding).
+
+    packed=True: no padding at all -- the sequences (BOS + bytes each) are laid end to end in packs of at most `max_tokens`
+    tokens (`packs`) and each pack is one model.score_tokens_packed call; `batch_size` does not apply."""
     from .scoring import score_sequences
     scores: List[float] = [0.0] * len(seqs)
+    if packed:
+        if reduce_method not in ("mean", "sum"):
+            raise ValueError(f"Invalid reduce_method {reduce_method}")
+        if any(len(s) == 0 for s in seqs):
+            raise ValueError("packed scoring: empty sequence")
+        reduce = np.mean if reduce_method == "mean" else np.sum
+        for rows, cu in packs([len(s) for s in seqs], max_tokens):
+            ids = packed_ids([seqs[i] for i in rows], tokenizer, device=device)
+            lp = model.score_tokens_packed(ids, cu, want_logprobs=True)[0].cpu().numpy()
+            for k, i in enumerate(rows):
+                scores[i] = float(reduce(lp[cu[k]:cu[k + 1] - 1]))
+        return scores
     for idx in length_buckets(seqs, batch_size=batch_size, mode="sorted", max_tokens=max_tokens):
         got = score_sequences([seqs[i] for i in idx], model, tokenizer, reduce_method=reduce_method, device=device)
         for i, g in zip(idx, got):

@@ -183,7 +183,7 @@ class Generator:
         return picked[:, :done], kept_logits[:, :done], state
 
 
-def _generate_ragged(prompt_seqs, model, tokenizer, engine, n_tokens, prepend_bos, batch_size, verbose):
+def _generate_ragged(prompt_seqs, model, tokenizer, engine, n_tokens, prepend_bos, batch_size, verbose, packed_prefill=False):
     """generate(ragged=True): prompts sorted by length and cut into batches of <= batch_size; per batch one ragged prefill
     (StripedHyena.prefill_ragged), one first pick (evo_sample) and one on-device loop with per-row positions.  Texts and
     scores come back in input order."""
@@ -212,7 +212,7 @@ def _generate_ragged(prompt_seqs, model, tokenizer, engine, n_tokens, prepend_bo
         picked = torch.empty(len(rows), n_tokens, dtype=torch.long, device=dev)
         kept_logits = torch.empty(len(rows), n_tokens, V, dtype=torch.float, device=dev)
         with torch.inference_mode():
-            head, state = model.prefill_ragged([ids[r] for r in rows], cache_len)
+            head, state = model.prefill_ragged([ids[r] for r in rows], cache_len, packed=packed_prefill)
         token = engine._pick_device(head)
         kept_logits[:, 0], picked[:, 0] = head, token
         if n_tokens > 1:
@@ -233,7 +233,7 @@ def _generate_ragged(prompt_seqs, model, tokenizer, engine, n_tokens, prepend_bo
 def generate(prompt_seqs: List[str], model, tokenizer: CharLevelTokenizer, n_tokens: int = 100, temperature: float = 0.0,
              top_k: int = 1, top_p: float = 1.0, batched: bool = True, prepend_bos: bool = False,
              cached_generation: bool = False, force_prompt_threshold: int = 128, verbose: int = 1,
-             device: str = "cuda:0", ragged: bool = False, batch_size: int = 64, **kwargs) -> Tuple[List[str], List[float]]:
+             device: str = "cuda:0", ragged: bool = False, batch_size: int = 64, packed_prefill: bool = False, **kwargs) -> Tuple[List[str], List[float]]:
     """Sequences and mean log-likelihood "scores" for a list of prompts.  Prompts of one common
     length run as one batch; anything else falls back to one prompt at a time (with a note on stderr).
 
@@ -241,7 +241,9 @@ def generate(prompt_seqs: List[str], model, tokenizer: CharLevelTokenizer, n_tok
     `batch_size` (64 keeps the stream-K decode GEMMs; larger batches take the 128x64 tiles), and each batch decodes with a
     position per row.  Every prompt is prefilled whole, so `force_prompt_threshold` does not apply and the reference's
     jump to the full prompt length (Q1) never happens.  Needs cached_generation=True, a CUDA model, non-empty prompts no
-    longer than the model's max_seqlen, and n_tokens >= 1; texts and scores come back in input order."""
+    longer than the model's max_seqlen, and n_tokens >= 1; texts and scores come back in input order.  packed_prefill=True
+    prefills each batch with one packed forward (StripedHyena.prefill_ragged(packed=True)) instead of one forward per
+    distinct prompt length."""
     model.eval()
     engine = Generator(model, tokenizer, top_k=top_k, top_p=top_p, temperature=temperature)
     if ragged:
@@ -249,7 +251,8 @@ def generate(prompt_seqs: List[str], model, tokenizer: CharLevelTokenizer, n_tok
             raise ValueError("ragged generation needs cached_generation=True")
         if batch_size < 1:
             raise ValueError("batch_size must be >= 1")
-        texts, scores = _generate_ragged(list(prompt_seqs), model, tokenizer, engine, int(n_tokens), prepend_bos, int(batch_size), verbose)
+        texts, scores = _generate_ragged(list(prompt_seqs), model, tokenizer, engine, int(n_tokens), prepend_bos, int(batch_size), verbose,
+                                         packed_prefill=bool(packed_prefill))
         if verbose:
             for prompt, text, score in zip(prompt_seqs, texts, scores):
                 print(f'Prompt: "{prompt}",\tOutput: "{text}",\tScore: {score}')

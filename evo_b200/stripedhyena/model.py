@@ -23,8 +23,8 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from .. import _lib
-from .._lib import (EPI_BIAS, EPI_BIAS_RESID, EPI_BIAS_ROPE, EPI_GELU_GATE, EPI_HYENA_STEP, EPI_NONE, EPI_RESID, AttnParams, GemmParams,
-                    GemmSmallMParams, HyenaParams, check, ptr)
+from .._lib import (EPI_BIAS, EPI_BIAS_RESID, EPI_BIAS_ROPE, EPI_GELU_GATE, EPI_HYENA_STEP, EPI_NONE, EPI_RESID, AttnParams, AttnVarlenParams,
+                    GemmParams, GemmSmallMParams, HyenaParams, HyenaVarlenParams, check, ptr)
 from .cache import InferenceParams, RecurrentInferenceParams
 
 # kernel variants (see include/evo_b200.h); overridable for experiments
@@ -35,6 +35,22 @@ ATTN_VARIANT = int(os.environ.get("EVO_B200_ATTN_VARIANT", "2"))
 
 def _round_up(x: int, m: int) -> int:
     return (x + m - 1) // m * m
+
+
+def packed_lengths(cu_seqlens, T: int):
+    """Host check of a packed batch's sequence boundaries (flash-attn varlen convention): cu_seqlens holds n + 1 offsets,
+    cu[0] = 0, strictly increasing (no empty sequence), cu[n] = T.  Returns the n lengths; raises EvoError otherwise."""
+    cu = [int(c) for c in (cu_seqlens.tolist() if torch.is_tensor(cu_seqlens) else cu_seqlens)]
+    if len(cu) < 2 or cu[0] != 0:
+        raise _lib.EvoError(f"cu_seqlens must hold n + 1 >= 2 offsets starting at 0, got {cu[:4]}")
+    lengths = [b - a for a, b in zip(cu[:-1], cu[1:])]
+    if min(lengths) <= 0:
+        raise _lib.EvoError(f"cu_seqlens must be strictly increasing (every sequence non-empty); sequence {lengths.index(min(lengths))} has length {min(lengths)}")
+    if cu[-1] != T:
+        raise _lib.EvoError(f"cu_seqlens ends at {cu[-1]}, the packed ids hold {T} tokens")
+    if len(lengths) > 65535:
+        raise _lib.EvoError(f"{len(lengths)} sequences in one pack; at most 65535")
+    return lengths
 
 
 # ----------------------------------------------------------------------------- parameter carriers
@@ -377,7 +393,7 @@ class StripedHyena(nn.Module):
         self._gemm(g, pk["w3"], out, M, d, pk["ipad"], EPI_RESID, resid=u)
         return out
 
-    def _hyena_block(self, i, blk, u, B, L, ip: Optional[RecurrentInferenceParams]):
+    def _hyena_block(self, i, blk, u, B, L, ip: Optional[RecurrentInferenceParams], varlen=None):
         cfg = self.config
         d, H = cfg.hidden_size, cfg.num_attention_heads
         M = B * L
@@ -390,7 +406,9 @@ class StripedHyena(nn.Module):
         y = xn  # (M, D) buffer reuse
         lib = _lib.lib()
         have_state = ip is not None and i in ip.fir_state_dict
-        if have_state and L == 1:
+        if varlen is not None:
+            self._hyena_varlen(i, f, z, y, varlen, ip)
+        elif have_state and L == 1:
             st = ip.state_dict[i]
             if not st.is_contiguous():
                 st = st.contiguous(); ip.state_dict[i] = st
@@ -424,7 +442,28 @@ class StripedHyena(nn.Module):
         self._gemm(y, blk.out_filter_dense.weight, u2, M, d, d, EPI_BIAS_RESID, bias=blk.out_filter_dense.bias, resid=u)
         return self._mlp_residual(i, blk, u2, M)
 
-    def _attention_block(self, i, blk, u, B, L, ip: Optional[InferenceParams]):
+    def _hyena_varlen(self, i, f, z, y, vl, ip):
+        """Packed sequences: one scan over all T rows (evo_hyena_fwd_varlen); with `ip`, each sequence's end states become
+        state_dict[i] (n, D, S) and fir_state_dict[i] (n, 3D, 2) as they are."""
+        cfg = self.config
+        d, n = cfg.hidden_size, vl["n"]
+        lib = _lib.lib()
+        hp = HyenaVarlenParams(z=z.data_ptr(), y=y.data_ptr(), fir_w=f.short_filter_weight.data_ptr(), fir_b=f.short_filter_bias.data_ptr(),
+                               Dskip=f.D.data_ptr(), poles=f.poles.data_ptr(), residues=f.residues.data_ptr(),
+                               cu_seqlens=vl["cu"].data_ptr(), n_seq=n, T=vl["T"], max_seqlen=vl["max"],
+                               D=d, S=cfg.state_size, nheads=cfg.num_attention_heads, seg_len=0)
+        if ip is not None:
+            st_out = torch.empty(n, d, cfg.state_size, 2, dtype=torch.float32, device=z.device)
+            fs_out = torch.empty(n, 3 * d, 2, dtype=torch.bfloat16, device=z.device)
+            hp.state_out, hp.fir_state_out = st_out.data_ptr(), fs_out.data_ptr()
+        ws_bytes = lib.evo_hyena_fwd_varlen_workspace(C.byref(hp))
+        ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=z.device)
+        self._record("hyena", 8.0 * vl["T"] * d, lambda: check(lib.evo_hyena_fwd_varlen(C.byref(hp), ptr(ws), ws_bytes, self._stream()), "evo_hyena_fwd_varlen"))
+        if ip is not None:
+            ip.state_dict[i] = torch.view_as_complex(st_out)
+            ip.fir_state_dict[i] = fs_out
+
+    def _attention_block(self, i, blk, u, B, L, ip: Optional[InferenceParams], varlen=None):
         cfg = self.config
         d, H = cfg.hidden_size, cfg.num_attention_heads
         hd = d // H
@@ -436,9 +475,12 @@ class StripedHyena(nn.Module):
         self._rmsnorm(u, blk.pre_norm.scale, xn, M)
         qkv = torch.empty(M, 3 * d, dtype=torch.bfloat16, device=dev)
         off = int(ip.seqlen_offset) if ip is not None else 0
-        cos, sin = self._rope_tables(off + L, dev)
-        hd2 = hd // 2
-        cos_p, sin_p = cos.data_ptr() + off * hd2 * 2, sin.data_ptr() + off * hd2 * 2
+        if varlen is not None:      # (T, 64) table of each row's in-sequence position: row m uses row m % rope_L, rope_L = T
+            cos_p, sin_p = (t.data_ptr() for t in varlen["rope"])
+        else:
+            cos, sin = self._rope_tables(off + L, dev)
+            hd2 = hd // 2
+            cos_p, sin_p = cos.data_ptr() + off * hd2 * 2, sin.data_ptr() + off * hd2 * 2
         if self.fused_rope and mha.Wqkv.bias is not None and hd == 128 and self.gemm_variant in (0, 1):
             # rotary applied in the projection's epilogue, where flash_attn's MHA applies it (mha.py:635-648): no second pass over qkv
             self._gemm(xn, mha.Wqkv.weight, qkv, M, 3 * d, d, EPI_BIAS_ROPE, bias=mha.Wqkv.bias, rope=(cos_p, sin_p, L, 2 * d))
@@ -446,6 +488,12 @@ class StripedHyena(nn.Module):
             self._gemm(xn, mha.Wqkv.weight, qkv, M, 3 * d, d, EPI_BIAS if mha.Wqkv.bias is not None else EPI_NONE, bias=mha.Wqkv.bias)
             self._record("rotary", 8.0 * M * d, lambda: check(lib.evo_rotary_qk(ptr(qkv), C.c_void_p(cos_p), C.c_void_p(sin_p), B, L, H, hd, self._stream()), "evo_rotary_qk"))
         ctx = xn  # reuse
+        if varlen is not None:
+            self._attention_varlen(i, qkv, ctx, varlen, ip)
+            u2 = torch.empty_like(u)
+            self._gemm(ctx, mha.out_proj.weight, u2, M, d, d, EPI_BIAS_RESID if mha.out_proj.bias is not None else EPI_RESID,
+                       bias=mha.out_proj.bias, resid=u)
+            return self._mlp_residual(i, blk, u2, M)
         ap = AttnParams(out=ctx.data_ptr(), B=B, Lq=L, H=H, hd=hd, q_pos0=off, softmax_scale=1.0 / math.sqrt(hd))
         ap.q, ap.q_tok_stride, ap.q_batch_stride = qkv.data_ptr(), 3 * d, L * 3 * d
         if ip is None:
@@ -468,6 +516,27 @@ class StripedHyena(nn.Module):
         self._gemm(ctx, mha.out_proj.weight, u2, M, d, d, EPI_BIAS_RESID if mha.out_proj.bias is not None else EPI_RESID,
                    bias=mha.out_proj.bias, resid=u)
         return self._mlp_residual(i, blk, u2, M)
+
+    def _attention_varlen(self, i, qkv, ctx, vl, ip):
+        """Packed sequences: causal attention within each sequence (evo_attn_fwd_varlen) on the packed qkv rows; with `ip`,
+        sequence b's k, v also go to rows [0, len_b) of batch row b of the layer's KV cache (evo_kv_append_varlen)."""
+        cfg = self.config
+        d, H = cfg.hidden_size, cfg.num_attention_heads
+        hd = d // H
+        lib = _lib.lib()
+        cu, n, T, mx = vl["cu"], vl["n"], vl["T"], vl["max"]
+        if ip is not None:
+            if i not in ip.key_value_memory_dict:
+                ip.key_value_memory_dict[i] = torch.zeros(max(ip.max_batch_size, n), ip.max_seqlen, 2, H, hd, dtype=torch.bfloat16, device=qkv.device)
+            cache = ip.key_value_memory_dict[i]
+            if n > cache.shape[0] or mx > cache.shape[1] or not cache.is_contiguous():
+                raise _lib.EvoError(f"KV cache {tuple(cache.shape)} cannot hold {n} sequences of up to {mx} tokens")
+            check(lib.evo_kv_append_varlen(ptr(qkv), ptr(cache), ptr(cu), n, T, mx, H, hd, cache.shape[1], self._stream()), "evo_kv_append_varlen")
+        ap = AttnVarlenParams(q=qkv.data_ptr(), k=qkv.data_ptr() + d * 2, v=qkv.data_ptr() + 2 * d * 2, out=ctx.data_ptr(),
+                              q_tok_stride=3 * d, kv_tok_stride=3 * d, cu_seqlens=cu.data_ptr(), n_seq=n, T=T, max_seqlen=mx,
+                              H=H, hd=hd, softmax_scale=1.0 / math.sqrt(hd))
+        causal_flops = 4.0 * H * hd * sum(L * (L + 1) / 2.0 for L in vl["lengths"])
+        self._record("attn", causal_flops, lambda: check(lib.evo_attn_fwd_varlen(C.byref(ap), self._stream()), "evo_attn_fwd_varlen"))
 
     # ---- forward ---------------------------------------------------------------------------------
     def forward(self, x, inference_params_dict=None, padding_mask=None):
@@ -495,8 +564,9 @@ class StripedHyena(nn.Module):
             self._gemm(u, self.unembed.weight, logits, M, V, d, EPI_NONE)
         return logits.view(B, L, V), inference_params_dict
 
-    def _backbone(self, x, B, L, inference_params_dict=None):
-        """embed -> all blocks -> final norm: the (B*L, D) bf16 input of the unembedding."""
+    def _backbone(self, x, B, L, inference_params_dict=None, varlen=None):
+        """embed -> all blocks -> final norm: the (B*L, D) bf16 input of the unembedding.  varlen (from _varlen): x is a packed
+        (T,) batch run as B = 1, L = T; only the two token-mixing calls differ."""
         M, d, V = B * L, self.config.hidden_size, self.config.vocab_size
         dev = x.device
         u = torch.empty(M, d, dtype=torch.bfloat16, device=dev)
@@ -505,10 +575,10 @@ class StripedHyena(nn.Module):
         for i, blk in enumerate(self.blocks):
             if i in self._attn_idxs:
                 ip = inference_params_dict["mha"] if inference_params_dict is not None else None
-                u = self._attention_block(i, blk, u, B, L, ip)
+                u = self._attention_block(i, blk, u, B, L, ip, varlen)
             else:
                 ip = inference_params_dict["hyena"] if inference_params_dict is not None else None
-                u = self._hyena_block(i, blk, u, B, L, ip)
+                u = self._hyena_block(i, blk, u, B, L, ip, varlen)
         if self.norm is not None:
             xn = torch.empty_like(u)
             self._rmsnorm(u, self.norm.scale, xn, M)
@@ -535,14 +605,72 @@ class StripedHyena(nn.Module):
             u = self._backbone(x, B, L, None)
             targets = torch.full((B, L), -1, dtype=torch.long, device=dev)
             targets[:, :-1] = x[:, 1:]
-            lp = torch.empty(B, L, dtype=torch.float32, device=dev) if want_logprobs else None
-            ent = torch.empty(B, L, dtype=torch.float32, device=dev) if want_entropy else None
-            n = lib.evo_unembed_score_workspace(M, V)
-            ws = torch.empty(max(n, 1), dtype=torch.uint8, device=dev)
-            sp = _lib.ScoreParams(x=u.data_ptr(), W=self.unembed.weight.data_ptr(), targets=targets.data_ptr(), logprobs=lp.data_ptr() if lp is not None else None,
-                                  entropy=ent.data_ptr() if ent is not None else None, M=M, V=V, K=d, workspace=ws.data_ptr(), workspace_bytes=n)
-            self._record(f"gemm/{V}x{d}/score", 2.0 * M * V * d, lambda: check(lib.evo_unembed_score(C.byref(sp), self._stream()), "evo_unembed_score"))
+            return self._score_head(u, targets, (B, L), want_logprobs, want_entropy)
+
+    def _score_head(self, u, targets, shape, want_logprobs, want_entropy):
+        """evo_unembed_score over the rows of u (the final-norm output): (logprobs, entropy) of `shape`, either None if unwanted."""
+        d, V = self.config.hidden_size, self.config.vocab_size
+        M, dev, lib = u.shape[0], u.device, _lib.lib()
+        lp = torch.empty(shape, dtype=torch.float32, device=dev) if want_logprobs else None
+        ent = torch.empty(shape, dtype=torch.float32, device=dev) if want_entropy else None
+        n = lib.evo_unembed_score_workspace(M, V)
+        ws = torch.empty(max(n, 1), dtype=torch.uint8, device=dev)
+        sp = _lib.ScoreParams(x=u.data_ptr(), W=self.unembed.weight.data_ptr(), targets=targets.data_ptr(), logprobs=lp.data_ptr() if lp is not None else None,
+                              entropy=ent.data_ptr() if ent is not None else None, M=M, V=V, K=d, workspace=ws.data_ptr(), workspace_bytes=n)
+        self._record(f"gemm/{V}x{d}/score", 2.0 * M * V * d, lambda: check(lib.evo_unembed_score(C.byref(sp), self._stream()), "evo_unembed_score"))
         return lp, ent
+
+    # ---- packed variable-length sequences: n sequences end to end as one (T,) batch, no padding ----------------------
+    def _varlen(self, ids, cu_seqlens):
+        """Checks a packed call on the host before anything is launched and returns what its blocks need: the device
+        cu_seqlens, n, T, the longest length, the lengths, and the (T, 64) rotary tables gathered at each row's position
+        inside its sequence (built once per forward, shared by every attention layer)."""
+        cfg = self.config
+        d, H = cfg.hidden_size, cfg.num_attention_heads
+        if d % H or d // H != 128 or d % 256:
+            raise _lib.EvoError(f"packed sequences need head_dim 128 and hidden_size % 256 == 0 (hidden_size {d}, {H} heads)")
+        if not torch.is_tensor(ids) or ids.dim() != 1 or ids.dtype not in (torch.int32, torch.int64):
+            raise _lib.EvoError("packed ids must be a 1-D int32/int64 tensor")
+        self._ensure_packed()
+        dev = self.embedding_layer.weight.device
+        if ids.device != dev:
+            raise _lib.EvoError(f"input ids on {ids.device}, model on {dev}")
+        T = ids.shape[0]
+        lengths = packed_lengths(cu_seqlens, T)
+        cu = torch.tensor([0] + lengths, dtype=torch.int64).cumsum_(0).to(dev)
+        vl = {"cu": cu, "n": len(lengths), "T": T, "max": max(lengths), "lengths": lengths, "rope": None}
+        if self._attn_idxs:
+            with torch.cuda.device(dev):
+                cos, sin = self._rope_tables(vl["max"], dev)
+                pos = torch.arange(T, device=dev) - torch.repeat_interleave(cu[:-1], torch.tensor(lengths, device=dev), output_size=T)
+                vl["rope"] = (cos[pos].contiguous(), sin[pos].contiguous())
+        return vl
+
+    def forward_packed(self, ids, cu_seqlens):
+        """Logits (T, V) bf16 of n sequences packed end to end: ids (T,), cu_seqlens n + 1 offsets (cu[0] = 0, cu[n] = T, no
+        empty sequence).  Row r holds what `forward` gives at that token of its sequence alone; equal lengths give the bits of
+        `forward` on the (n, L) batch.  One backbone pass over T rows: no padding, one GEMM of M = T per linear layer."""
+        vl = self._varlen(ids, cu_seqlens)
+        d, V = self.config.hidden_size, self.config.vocab_size
+        dev, T = ids.device, vl["T"]
+        with torch.cuda.device(dev), torch.no_grad():
+            u = self._backbone(ids.contiguous(), 1, T, None, vl)
+            logits = torch.empty(T, V, dtype=torch.bfloat16, device=dev)
+            self._gemm(u, self.unembed.weight, logits, T, V, d, EPI_NONE)
+        return logits
+
+    def score_tokens_packed(self, ids, cu_seqlens, want_logprobs=True, want_entropy=False):
+        """score_tokens for packed sequences: (logprobs (T,) fp32 or None, entropy (T,) fp32 or None).  The target of row r is
+        the next token of the same sequence; the last row of each sequence has none (logprob 0)."""
+        vl = self._varlen(ids, cu_seqlens)
+        dev, T = ids.device, vl["T"]
+        x = ids.contiguous()
+        with torch.cuda.device(dev), torch.no_grad():
+            u = self._backbone(x, 1, T, None, vl)
+            targets = torch.empty(T, dtype=torch.long, device=dev)
+            targets[:-1] = x[1:]
+            targets[vl["cu"][1:] - 1] = -1
+            return self._score_head(u, targets, (T,), want_logprobs, want_entropy)
 
     # ---- decode step: small-M weight-streaming GEMM tiles + device-side position + CUDA graph ------
     def _can_step(self, ipd, B):
@@ -667,8 +795,13 @@ class StripedHyena(nn.Module):
         return logits
 
     # ---- prefill of prompts of different lengths into one decode batch ------------------------------------------------
-    def prefill_ragged(self, prompts, cache_len):
+    def prefill_ragged(self, prompts, cache_len, packed=False):
         """Prefill B prompts of different lengths into one state that decode_loop steps with per-row positions.
+
+        packed=True: one packed forward over all prompts end to end (forward_packed's path with state emission): the KV
+        caches are written by evo_kv_append_varlen, each prompt's Hyena end states come straight out of the varlen scan, and
+        only the B last rows are unembedded.  Rows may then be in any order.  Equal-length prompts give the grouped path's
+        bits.  Otherwise:
 
         prompts: B non-empty 1-D token sequences (lists or int tensors); rows of equal length must be adjacent (sort by
         length).  The rows are grouped by exact length (frontend.length_buckets) and each group runs the stateful forward
@@ -681,6 +814,8 @@ class StripedHyena(nn.Module):
         cfg = self.config
         B = len(prompts)
         lengths = [len(p) for p in prompts]
+        if packed:
+            return self._prefill_packed(prompts, lengths, cache_len)
         if B == 0 or min(lengths) == 0:
             raise ValueError("prefill_ragged needs at least one prompt and no empty prompt")
         if max(lengths) > cache_len:
@@ -712,6 +847,29 @@ class StripedHyena(nn.Module):
             hy.fir_state_dict = {i: torch.cat(v, 0) for i, v in fir.items()}
             mha = InferenceParams(max_seqlen=cache_len, max_batch_size=B, seqlen_offset=0, key_value_memory_dict=caches,
                                   lengths_per_sample=torch.tensor(lengths, dtype=torch.int64, device=dev))
+        return head, {"mha": mha, "hyena": hy}
+
+    def _prefill_packed(self, prompts, lengths, cache_len):
+        cfg = self.config
+        B = len(prompts)
+        d, H, V = cfg.hidden_size, cfg.num_attention_heads, cfg.vocab_size
+        if lengths and max(lengths) > cache_len:
+            raise _lib.EvoError(f"prompt length {max(lengths)} exceeds the KV cache ({cache_len})")
+        cu = [0]
+        for n in lengths:
+            cu.append(cu[-1] + n)
+        dev = self.embedding_layer.weight.device
+        ids = torch.cat([torch.as_tensor(p, dtype=torch.long) for p in prompts] or [torch.zeros(0, dtype=torch.long)]).to(dev)
+        vl = self._varlen(ids, cu)          # raises on an empty prompt, before anything is launched
+        with torch.cuda.device(dev), torch.no_grad():
+            caches = {i: torch.zeros(B, cache_len, 2, H, d // H, dtype=torch.bfloat16, device=dev) for i in sorted(self._attn_idxs)}
+            mha = InferenceParams(max_seqlen=cache_len, max_batch_size=B, seqlen_offset=0, key_value_memory_dict=caches,
+                                  lengths_per_sample=torch.tensor(lengths, dtype=torch.int64, device=dev))
+            hy = RecurrentInferenceParams(fir_filter_length=cfg.short_filter_length, state_dim=cfg.state_size, seqlen_offset=0)
+            u = self._backbone(ids, 1, vl["T"], {"mha": mha, "hyena": hy}, vl)
+            last = u.index_select(0, vl["cu"][1:] - 1)
+            head = torch.empty(B, V, dtype=torch.bfloat16, device=dev)
+            self._gemm(last, self.unembed.weight, head, B, V, d, EPI_NONE)      # the full-logits unembed's variant: the same bits per row
         return head, {"mha": mha, "hyena": hy}
 
     # ---- on-device generation loop (SURVEY 8f-2): token pick + bookkeeping + feedback inside the captured step ------

@@ -144,6 +144,27 @@ typedef struct {
 size_t evo_hyena_fwd_workspace(const evo_hyena_params* p);
 int evo_hyena_fwd(const evo_hyena_params* p, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- packed variable-length forward (flash-attn varlen convention) ----
+ * n_seq sequences laid end to end as T rows; cu_seqlens: (n_seq + 1) int64 DEVICE array, cu[0] = 0, cu[n_seq] = T, every
+ * sequence non-empty; max_seqlen = the longest length.  Each kernel clamps sequence b's rows to [0, T) and its length to
+ * max_seqlen, so a malformed device array cannot move a load or store out of bounds.
+ * evo_hyena_fwd_varlen: z (T, 3D) -> y (T, D), the mode-split scan only (head_dim 128, D % 256 == 0); every sequence starts
+ *   from zero state and zero FIR history.  Optional state_out (n_seq, D, S, 2) fp32 and fir_state_out (n_seq, 3D, 2) bf16:
+ *   each sequence's end states.  seg_len: 0 = automatic (nseg = the segment count evo_hyena_fwd picks for an (n_seq,
+ *   max_seqlen) batch, seg_len = ceil(max_seqlen / nseg): on equal lengths the batched call's geometry and bits);
+ *   > 0 forces it (tests).  workspace: evo_hyena_fwd_varlen_workspace() bytes. */
+typedef struct {
+  const void* z; void* y;
+  const void* fir_w; const void* fir_b; const void* Dskip;
+  const float* poles; const float* residues;
+  const int64_t* cu_seqlens; int n_seq; int64_t T, max_seqlen;
+  int D; int S; int nheads;
+  float* state_out; void* fir_state_out;
+  int64_t seg_len;
+} evo_hyena_varlen_params;
+size_t evo_hyena_fwd_varlen_workspace(const evo_hyena_varlen_params* p);
+int evo_hyena_fwd_varlen(const evo_hyena_varlen_params* p, void* workspace, size_t workspace_bytes, void* stream);
+
 /* decode step: engine.step_fir + step_iir.  u (B, 3D) bf16 -> y (B, D) bf16;
  * fir_state (B, 3D, 2) bf16 and state (B, D, S, 2) fp32 are updated in place. */
 int evo_hyena_step(const void* u, void* y, void* fir_state, float* state,
@@ -195,10 +216,26 @@ typedef struct {
 size_t evo_attn_fwd_workspace(const evo_attn_params* p, int variant);
 int evo_attn_fwd_ws(const evo_attn_params* p, int variant, void* workspace, size_t workspace_bytes, void* stream);
 
+/* packed causal attention (see evo_hyena_fwd_varlen for cu_seqlens): q, k, v (T, H, 128) with q_tok_stride / kv_tok_stride
+ * elements between tokens; out (T, H*128).  Sequence b attends within rows [cu[b], cu[b+1]) only; its output is the bits of
+ * a batch-1 evo_attn_fwd_ws call on that sequence. */
+typedef struct {
+  const void* q; const void* k; const void* v; void* out;
+  int64_t q_tok_stride, kv_tok_stride;
+  const int64_t* cu_seqlens; int n_seq; int64_t T, max_seqlen;
+  int H; int hd;
+  float softmax_scale;
+} evo_attn_varlen_params;
+int evo_attn_fwd_varlen(const evo_attn_varlen_params* p, void* stream);
+
 /* append k,v of qkv (B, L, 3, H, hd) at rows [pos0, pos0+L) of the KV cache
  * (max_B, max_seqlen, 2, H, hd) bf16 — MHA._update_kv_cache (mha.py:344-370). */
 int evo_kv_append(const void* qkv, void* cache, int B, int64_t L, int H, int hd,
                   int64_t pos0, int64_t max_seqlen, void* stream);
+/* packed form: k,v of packed qkv (T, 3, H, hd) rows [cu[b], cu[b+1]) go to cache rows [0, len_b) of batch row b of the cache
+ * (n_seq, cache_len, 2, H, hd); max_seqlen (the longest sequence) <= cache_len. */
+int evo_kv_append_varlen(const void* qkv, void* cache, const int64_t* cu_seqlens, int n_seq, int64_t T, int64_t max_seqlen,
+                         int H, int hd, int64_t cache_len, void* stream);
 
 /* ---- decode step (L == 1), CUDA-graph friendly: the sequence position is read from DEVICE memory ----
  * evo_gelu_gate_interleaved: out[m, g*128+c] = bf16(gelu(t[m, g*256+c])) * t[m, g*256+128+c]; t (M, 2*ipad) is the

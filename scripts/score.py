@@ -9,7 +9,8 @@ Scores the sequences of a FASTA file (mean log-likelihood per nucleotide) and wr
 Same arguments as the reference's scripts/score.py; what runs underneath is the evo_b200 engine: FASTA read without
 Biopython (evo_b200.frontend.read_fasta), sequences scored in LENGTH BUCKETS (--batch-size sequences or --max-tokens padded
 tokens per batch, whichever is hit first; the reference pads every file-order batch to its longest member), scores returned
-in file order.  --random-init / --model-dir are for boxes without network.
+in file order.  --packed lays the sequences end to end without any padding instead (packs of --max-tokens tokens, one
+forward each).  --random-init / --model-dir are for boxes without network.
 """
 import argparse
 
@@ -26,6 +27,7 @@ def build_parser():
     parser.add_argument('--model-name', type=str, default='evo-1-131k-base', help='Evo model name')
     parser.add_argument('--batch-size', type=int, default=32, help='Number of sequences to evaluate at a time')
     parser.add_argument('--max-tokens', type=int, default=1 << 17, help='Padded tokens per batch (bounds the activation footprint)')
+    parser.add_argument('--packed', action='store_true', help='Score sequences packed end to end (no padding) in packs of --max-tokens tokens')
     parser.add_argument('--device', type=str, default='cuda:0', help='Device for scoring')
     parser.add_argument('--random-init', action='store_true', help='Skip the checkpoint download (random weights; smoke runs offline)')
     parser.add_argument('--model-dir', type=str, default=None, help='Directory of an already downloaded HF snapshot')
@@ -39,7 +41,8 @@ def main(argv=None):
     model.eval()
     _, seqs = read_fasta(args.input_fasta)
     print(f'Scoring {len(seqs)} sequences...')
-    scores = score_many(seqs, model, tokenizer, batch_size=args.batch_size, max_tokens=args.max_tokens, device=args.device)
+    scores = score_many(seqs, model, tokenizer, batch_size=args.batch_size, max_tokens=args.max_tokens, device=args.device,
+                        packed=args.packed)
     with open(args.output_tsv, 'w') as f:
         f.write('seqs\tscores\n')
         for s, v in zip(seqs, scores):
