@@ -117,6 +117,10 @@ SIGNATURES = {
     "evo_decode_qkv_prep_rows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int64, C.c_void_p]),
     "evo_decode_attn_rows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int64, C.c_int, C.c_float, C.c_void_p, C.c_size_t, C.c_void_p]),
     "evo_advance_positions": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_void_p]),
+    "evo_decode_qkv_prep_shared": (C.c_int, [C.c_void_p] * 6 + [C.c_int, C.c_int, C.c_int, C.c_int64, C.c_void_p]),
+    "evo_decode_attn_shared_workspace": (C.c_size_t, [C.c_int, C.c_int, C.c_int, C.c_int]),
+    "evo_decode_attn_shared": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64,
+                                         C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_void_p, C.c_size_t, C.c_void_p]),
     "evo_sample": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, C.c_uint64, C.c_uint64, C.c_void_p]),
     "evo_sample_step": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "evo_advance_counters": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),

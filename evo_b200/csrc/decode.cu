@@ -3,6 +3,7 @@
 // serves every step (the reference re-launches ~20 tiny kernels per layer per token from
 // Python, SURVEY.md 8a row a9/a12).
 #include "common.cuh"
+#include "wgmma.cuh"
 #include "../../include/evo_b200.h"
 #include <cstdlib>
 
@@ -28,6 +29,25 @@ __global__ void gelu_gate_kernel(const bf16* __restrict__ t, bf16* __restrict__ 
   *reinterpret_cast<uint32_t*>(out + m * ipad + c2) = pack_bf16(o0, o1);
 }
 
+// Rotary on element pair (i, i + 64) of q,k of row b, head h at position `pos`; k,v appended at cache row `row`.
+__device__ __forceinline__ void qkv_prep_pair(bf16* __restrict__ qkv, bf16* __restrict__ cache, const bf16* __restrict__ cos, const bf16* __restrict__ sin,
+                                              long long pos, long long row, int b, int h, int i, int H, long long max_seqlen) {
+  const float c = __bfloat162float(cos[pos * 64 + i]), s = __bfloat162float(sin[pos * 64 + i]);
+  bf16* q = qkv + ((long long)(b * 3 + 0) * H + h) * HD;
+  bf16* k = qkv + ((long long)(b * 3 + 1) * H + h) * HD;
+  const bf16* v = qkv + ((long long)(b * 3 + 2) * H + h) * HD;
+  float q0 = __bfloat162float(q[i]), q1 = __bfloat162float(q[i + 64]);
+  float k0 = __bfloat162float(k[i]), k1 = __bfloat162float(k[i + 64]);
+  bf16 kr0 = __float2bfloat16_rn(k0 * c - k1 * s), kr1 = __float2bfloat16_rn(k0 * s + k1 * c);
+  q[i] = __float2bfloat16_rn(q0 * c - q1 * s);
+  q[i + 64] = __float2bfloat16_rn(q0 * s + q1 * c);
+  k[i] = kr0; k[i + 64] = kr1;
+  bf16* ck = cache + (((long long)b * max_seqlen + row) * 2 + 0) * H * HD + (long long)h * HD;
+  bf16* cv = ck + (long long)H * HD;
+  ck[i] = kr0; ck[i + 64] = kr1;
+  cv[i] = v[i]; cv[i + 64] = v[i + 64];
+}
+
 // L == 1: rotary on q,k at position pos_ptr[b * pos_stride], k,v appended to the cache at that row.  pos_stride 0 = one
 // position shared by the batch, 1 = one position per row (prompts of different lengths decoded together).
 // qkv (B, 3, H, 128) in place; cos/sin tables indexed by absolute position.
@@ -39,20 +59,20 @@ __global__ void decode_qkv_prep_kernel(bf16* __restrict__ qkv, bf16* __restrict_
   int i = idx % 64, h = (idx / 64) % H, b = idx / (64 * H);
   const long long pos = pos_ptr[(long long)b * pos_stride];
   if (pos >= max_seqlen) return;
-  const float c = __bfloat162float(cos[pos * 64 + i]), s = __bfloat162float(sin[pos * 64 + i]);
-  bf16* q = qkv + ((long long)(b * 3 + 0) * H + h) * HD;
-  bf16* k = qkv + ((long long)(b * 3 + 1) * H + h) * HD;
-  const bf16* v = qkv + ((long long)(b * 3 + 2) * H + h) * HD;
-  float q0 = __bfloat162float(q[i]), q1 = __bfloat162float(q[i + 64]);
-  float k0 = __bfloat162float(k[i]), k1 = __bfloat162float(k[i + 64]);
-  bf16 kr0 = __float2bfloat16_rn(k0 * c - k1 * s), kr1 = __float2bfloat16_rn(k0 * s + k1 * c);
-  q[i] = __float2bfloat16_rn(q0 * c - q1 * s);
-  q[i + 64] = __float2bfloat16_rn(q0 * s + q1 * c);
-  k[i] = kr0; k[i + 64] = kr1;
-  bf16* ck = cache + (((long long)b * max_seqlen + pos) * 2 + 0) * H * HD + (long long)h * HD;
-  bf16* cv = ck + (long long)H * HD;
-  ck[i] = kr0; ck[i + 64] = kr1;
-  cv[i] = v[i]; cv[i + 64] = v[i + 64];
+  qkv_prep_pair(qkv, cache, cos, sin, pos, pos, b, h, i, H, max_seqlen);
+}
+
+// Shared-prefix decode: rotary at the absolute position pos[b], k,v appended at row spos[b] of the row's own suffix cache
+// (B, S, 2, H, 128) that holds the generated tokens only.
+__global__ void decode_qkv_prep_shared_kernel(bf16* __restrict__ qkv, bf16* __restrict__ cache, const bf16* __restrict__ cos, const bf16* __restrict__ sin,
+                                              const long long* __restrict__ pos_ptr, const long long* __restrict__ spos_ptr, int B, int H, long long S) {
+  pdl_launch_dependents(); pdl_wait();
+  int idx = blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= B * H * 64) return;
+  int i = idx % 64, h = (idx / 64) % H, b = idx / (64 * H);
+  const long long pos = pos_ptr[b], row = spos_ptr[b];
+  if (row < 0 || row >= S || pos < 0) return;
+  qkv_prep_pair(qkv, cache, cos, sin, pos, row, b, h, i, H, S);
 }
 
 // Single-query attention over the KV cache, keys [0, pos_ptr[b * pos_stride]].  grid (H, B, nsplit); each CTA scans a
@@ -266,6 +286,203 @@ __global__ void decode_attn_merge_kernel(const float* __restrict__ part_o, const
   out[((long long)b * H + h) * HD + d] = __float2bfloat16_rn(acc / L);
 }
 
+// ---- shared-prefix decode attention: the prefix part ----
+// Rows of a group (samples of one prompt) are contiguous in the batch and share one prefix of K,V in a (G, P, 2, H, 128) cache.
+// One CTA = one head, one chunk of <= 64 rows of one group, one key split: the chunk's query rows are one m64 wgmma tile loaded
+// once by TMA straight from qkv (B, 3, H, 128); the split's keys stream through a 3-stage ring of 128-key K and V tiles, each read
+// once for all the chunk's rows.  S = Q K^T (wgmma m64n128k16, both operands in shared memory), an online softmax on the
+// fragments (fp32, exact running max), P rounded to bf16 straight into the A fragment of O += P V (V read in place as the
+// MN-major operand).  Every prefix key is visible (no causal mask); keys at or past prefix_len[g] are masked, and the V rows of
+// a tile past that point are zeroed in shared memory before the PV product, so whatever the cache holds there (NaN included)
+// cannot reach the output.  Output: unnormalised (m, l, o) per (row, head, split), m in natural-log units like the other
+// decode partials; rows of the tile outside the chunk are never stored.  warps 0-3: the consumer warpgroup; warp 4: producer.
+constexpr int SP_ROWS = 64;
+constexpr int SP_KEYS = 128;
+constexpr int SP_STAGES = 3;
+constexpr int SP_Q_BYTES = SP_ROWS * HD * 2;           // 2 x 64-column halves of 8 KB
+constexpr int SP_KV_BYTES = SP_KEYS * HD * 2;          // 2 x 64-column halves of 16 KB
+constexpr int SP_SMEM = SP_Q_BYTES + 2 * SP_STAGES * SP_KV_BYTES + 256;
+static_assert(SP_SMEM <= 232448, "exceeds the 227 KB dynamic shared memory limit");
+
+__device__ __forceinline__ float ex2f(float x) { float y; asm volatile("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
+
+__global__ void __launch_bounds__(160, 1) decode_attn_prefix_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmKV,
+                                                                    const long long* __restrict__ grp, const long long* __restrict__ plen_ptr,
+                                                                    int G, long long P, int B, int H, int nsplit, float scale_log2,
+                                                                    float* __restrict__ part_o, float* __restrict__ part_ml) {
+  pdl_launch_dependents(); pdl_wait();
+  extern __shared__ __align__(1024) uint8_t smem[];
+  if ((smem_u32(smem) & 1023u) != 0) __trap();                         // 128B-swizzled tiles need 1024-byte alignment
+  uint8_t* sQ = smem;
+  uint8_t* sK = sQ + SP_Q_BYTES;
+  uint8_t* sV = sK + SP_STAGES * SP_KV_BYTES;
+  uint64_t* q_full = reinterpret_cast<uint64_t*>(sV + SP_STAGES * SP_KV_BYTES);
+  uint64_t* k_full = q_full + 1;
+  uint64_t* k_empty = k_full + SP_STAGES;
+  uint64_t* v_full = k_empty + SP_STAGES;
+  uint64_t* v_empty = v_full + SP_STAGES;
+  const int h = blockIdx.x, sp = blockIdx.z, tid = threadIdx.x;
+
+  // blockIdx.y -> (group, 64-row chunk of it); offsets are clamped to [0, B] so a malformed array cannot move a load or store
+  int c = blockIdx.y, g = 0;
+  long long r0 = 0, nrows = 0;
+  for (; g < G; ++g) {
+    const long long a = min(max(grp[g], 0LL), (long long)B), e = min(max(grp[g + 1], a), (long long)B);
+    const long long nch = (e - a + SP_ROWS - 1) / SP_ROWS;
+    if (c < nch) { r0 = a + (long long)c * SP_ROWS; nrows = min((long long)SP_ROWS, e - r0); break; }
+    c -= (int)nch;
+  }
+  if (g == G) return;                                                   // past the last chunk: the grid is an upper bound
+  const long long plen = min(max(plen_ptr[g], 0LL), P);
+  long long per = (plen + nsplit - 1) / nsplit;
+  per = (per + SP_KEYS - 1) / SP_KEYS * SP_KEYS;                         // splits start on tile boundaries
+  const long long k0 = (long long)sp * per, k1 = min(plen, k0 + per);
+  const int ntiles = k1 > k0 ? (int)((k1 - k0 + SP_KEYS - 1) / SP_KEYS) : 0;
+
+  if (tid == 0) {
+    mbar_init(q_full, 1);
+    for (int i = 0; i < SP_STAGES; ++i) { mbar_init(&k_full[i], 1); mbar_init(&k_empty[i], 4); mbar_init(&v_full[i], 1); mbar_init(&v_empty[i], 4); }
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (tid >= 128) {
+    if (tid == 128 && ntiles > 0) {
+      tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmKV);
+      mbar_arrive_expect_tx(q_full, SP_Q_BYTES);
+      tma_load_3d(sQ, &tmQ, q_full, 0, h, (int)r0);
+      tma_load_3d(sQ + SP_Q_BYTES / 2, &tmQ, q_full, 64, h, (int)r0);
+      for (int t = 0; t < ntiles; ++t) {
+        const int st = t % SP_STAGES;
+        const uint32_t ph = (uint32_t)(t / SP_STAGES) & 1;
+        const int row = (int)((long long)g * P + k0 + (long long)t * SP_KEYS);
+        mbar_wait(&k_empty[st], ph ^ 1);
+        mbar_arrive_expect_tx(&k_full[st], SP_KV_BYTES);
+        tma_load_3d(sK + st * SP_KV_BYTES, &tmKV, &k_full[st], 0, h, row);
+        tma_load_3d(sK + st * SP_KV_BYTES + SP_KV_BYTES / 2, &tmKV, &k_full[st], 64, h, row);
+        mbar_wait(&v_empty[st], ph ^ 1);
+        mbar_arrive_expect_tx(&v_full[st], SP_KV_BYTES);
+        tma_load_3d(sV + st * SP_KV_BYTES, &tmKV, &v_full[st], 0, H + h, row);
+        tma_load_3d(sV + st * SP_KV_BYTES + SP_KV_BYTES / 2, &tmKV, &v_full[st], 64, H + h, row);
+      }
+    }
+    return;
+  }
+  const int warp = tid >> 5, lane = tid & 31, quad = lane & 3;
+  const int r = warp * 16 + (lane >> 2);                                // this thread's rows of the tile: r and r + 8
+  float o[HD / 2];
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+#pragma unroll
+  for (int i = 0; i < HD / 2; ++i) o[i] = 0.f;
+  if (ntiles > 0) mbar_wait(q_full, 0);
+  const uint32_t qa = smem_u32(sQ);
+  for (int t = 0; t < ntiles; ++t) {
+    const int st = t % SP_STAGES;
+    const uint32_t ph = (uint32_t)(t / SP_STAGES) & 1;
+    const long long key0 = k0 + (long long)t * SP_KEYS;
+    float s[SP_KEYS / 2];
+    mbar_wait(&k_full[st], ph);
+    const uint32_t ka = smem_u32(sK + st * SP_KV_BYTES);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < HD / 16; ++kk)
+      wgmma_m64n128k16_ss(s, wgmma_desc_k_sw128(qa + (kk >> 2) * (SP_Q_BYTES / 2) + (kk & 3) * 32),
+                          wgmma_desc_k_sw128(ka + (kk >> 2) * (SP_KV_BYTES / 2) + (kk & 3) * 32), kk != 0);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(s);
+    if (lane == 0) mbar_arrive(&k_empty[st]);
+    const bool partial = key0 + SP_KEYS > k1;                           // the split's last tile: keys at or past k1 are masked
+    if (partial) {
+#pragma unroll
+      for (int i = 0; i < SP_KEYS / 8; ++i)
+#pragma unroll
+        for (int e = 0; e < 2; ++e)
+          if (key0 + 8 * i + 2 * quad + e >= k1) { s[4 * i + e] = -INFINITY; s[4 * i + 2 + e] = -INFINITY; }
+    }
+    uint32_t pf[SP_KEYS / 16][4];
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) {
+      float mx = -INFINITY;
+#pragma unroll
+      for (int i = 0; i < SP_KEYS / 8; ++i) mx = fmaxf(mx, fmaxf(s[4 * i + 2 * hr], s[4 * i + 2 * hr + 1]));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2)) * scale_log2;
+      const float mn = fmaxf(m[hr], mx);                                // finite: every tile holds at least one visible key
+      const float alpha = ex2f(m[hr] - mn);
+      m[hr] = mn; l[hr] *= alpha;
+#pragma unroll
+      for (int i = 0; i < HD / 8; ++i) { o[4 * i + 2 * hr] *= alpha; o[4 * i + 2 * hr + 1] *= alpha; }
+      float ls = 0.f;
+#pragma unroll
+      for (int i = 0; i < SP_KEYS / 8; ++i) {
+        const float p0 = ex2f(fmaf(s[4 * i + 2 * hr], scale_log2, -mn));
+        const float p1 = ex2f(fmaf(s[4 * i + 2 * hr + 1], scale_log2, -mn));
+        ls += p0 + p1;
+        pf[i >> 1][(i & 1) * 2 + hr] = pack_bf16(p0, p1);               // P rounded to bf16 before the PV product
+      }
+      l[hr] += ls;
+    }
+    mbar_wait(&v_full[st], ph);
+    uint8_t* vs = sV + st * SP_KV_BYTES;
+    if (partial) {                                                      // zero V rows [k1 - key0, 128): a 128-byte swizzled row stays one row
+      const int nvalid = (int)(k1 - key0);
+      for (int idx = tid; idx < (SP_KEYS - nvalid) * 16; idx += 128) {
+        const int row = nvalid + idx / 16, chunk = idx % 16;
+        *reinterpret_cast<uint4*>(vs + (chunk / 8) * (SP_KV_BYTES / 2) + row * 128 + (chunk % 8) * 16) = make_uint4(0, 0, 0, 0);
+      }
+      fence_proxy_async_smem();
+      named_bar_sync(1, 128);
+    }
+    const uint32_t va = smem_u32(vs);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < SP_KEYS / 16; ++kk)
+      wgmma_m64n128k16_rs<1>(o, pf[kk], wgmma_desc_sw128(va + kk * 16 * 128, SP_KV_BYTES / 2, 1024), 1);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(o);
+    if (lane == 0) mbar_arrive(&v_empty[st]);
+  }
+#pragma unroll
+  for (int hr = 0; hr < 2; ++hr) {
+    float lt = l[hr];
+    lt += __shfl_xor_sync(0xffffffffu, lt, 1);
+    lt += __shfl_xor_sync(0xffffffffu, lt, 2);
+    if (r + 8 * hr >= nrows) continue;
+    const long long pidx = ((r0 + r + 8 * hr) * H + h) * nsplit + sp;
+    float* po = part_o + pidx * HD;
+#pragma unroll
+    for (int i = 0; i < HD / 8; ++i) *reinterpret_cast<float2*>(po + 8 * i + 2 * quad) = make_float2(o[4 * i + 2 * hr], o[4 * i + 2 * hr + 1]);
+    if (quad == 0) { part_ml[pidx * 2] = m[hr] * 0.69314718055994531f; part_ml[pidx * 2 + 1] = lt; }
+  }
+}
+
+// Two-source form of decode_attn_merge_kernel: the prefix partials (np splits) and the suffix partials (ns splits) of row b.
+__global__ void decode_attn_merge2_kernel(const float* __restrict__ p_o, const float* __restrict__ p_ml, int np,
+                                          const float* __restrict__ s_o, const float* __restrict__ s_ml, int ns, bf16* __restrict__ out, int H) {
+  pdl_launch_dependents(); pdl_wait();
+  const int h = blockIdx.x, b = blockIdx.y, d = threadIdx.x;
+  const long long bp = ((long long)b * H + h) * np, bs = ((long long)b * H + h) * ns;
+  float M = -INFINITY;
+  for (int s = 0; s < np; ++s) M = fmaxf(M, p_ml[(bp + s) * 2]);
+  for (int s = 0; s < ns; ++s) M = fmaxf(M, s_ml[(bs + s) * 2]);
+  float L = 0.f, acc = 0.f;
+  for (int s = 0; s < np; ++s) {
+    const float ms = p_ml[(bp + s) * 2];
+    const float w = (ms == -INFINITY) ? 0.f : __expf(ms - M);
+    L += p_ml[(bp + s) * 2 + 1] * w;
+    acc += p_o[(bp + s) * HD + d] * w;
+  }
+  for (int s = 0; s < ns; ++s) {
+    const float ms = s_ml[(bs + s) * 2];
+    const float w = (ms == -INFINITY) ? 0.f : __expf(ms - M);
+    L += s_ml[(bs + s) * 2 + 1] * w;
+    acc += s_o[(bs + s) * HD + d] * w;
+  }
+  out[((long long)b * H + h) * HD + d] = __float2bfloat16_rn(acc / L);
+}
+
 __global__ void add_i64_kernel(long long* p, long long v) { *p += v; }
 
 __global__ void add_i64_rows_kernel(long long* p, int n, long long v) {
@@ -305,13 +522,10 @@ extern "C" int evo_decode_qkv_prep_rows(void* qkv, void* cache, const void* cos,
 
 extern "C" size_t evo_decode_attn_workspace(int B, int H, int nsplit) { return (size_t)B * H * nsplit * (HD + 2) * sizeof(float); }
 
-static int decode_attn(const char* what, const void* qkv, const void* cache, void* out, const int64_t* pos, int pos_stride, int B, int H, int hd,
-                       int64_t max_seqlen, int nsplit, float softmax_scale, void* workspace, size_t workspace_bytes, void* stream) {
-  EVO_REQUIRE(hd == HD, "%s: head_dim %d unsupported", what, hd);
-  EVO_REQUIRE(nsplit >= 1 && nsplit <= 64, "%s: bad nsplit %d", what, nsplit);
-  EVO_REQUIRE(workspace && workspace_bytes >= evo_decode_attn_workspace(B, H, nsplit), "%s: workspace too small", what);
-  float* part_o = (float*)workspace;
-  float* part_ml = part_o + (size_t)B * H * nsplit * HD;
+// the split partials of one query per row over cache keys [0, pos[b * pos_stride]]: the TMA-fed kernel when the cache length is a
+// multiple of 64, the per-thread-row kernel otherwise
+static int decode_attn_partials(const char* what, const void* qkv, const void* cache, float* part_o, float* part_ml, const int64_t* pos, int pos_stride,
+                                int B, int H, int64_t max_seqlen, int nsplit, float softmax_scale, void* stream) {
   static const bool force_v1 = getenv("EVO_B200_DECODE_ATTN_V1") != nullptr;
   int rc;
   if (max_seqlen % TK == 0 && !force_v1 && (long long)B * max_seqlen < (1LL << 31)) {
@@ -329,7 +543,18 @@ static int decode_attn(const char* what, const void* qkv, const void* cache, voi
     EVO_CUDA(launch_pdl(decode_attn_kernel, dim3(H, B, nsplit), dim3(DT), 0, (cudaStream_t)stream, (const bf16*)qkv, (const bf16*)cache, part_o, part_ml,
                         (const long long*)pos, pos_stride, H, max_seqlen, nsplit, softmax_scale));
   }
-  if ((rc = check_launch(what))) return rc;
+  return check_launch(what);
+}
+
+static int decode_attn(const char* what, const void* qkv, const void* cache, void* out, const int64_t* pos, int pos_stride, int B, int H, int hd,
+                       int64_t max_seqlen, int nsplit, float softmax_scale, void* workspace, size_t workspace_bytes, void* stream) {
+  EVO_REQUIRE(hd == HD, "%s: head_dim %d unsupported", what, hd);
+  EVO_REQUIRE(nsplit >= 1 && nsplit <= 64, "%s: bad nsplit %d", what, nsplit);
+  EVO_REQUIRE(workspace && workspace_bytes >= evo_decode_attn_workspace(B, H, nsplit), "%s: workspace too small", what);
+  float* part_o = (float*)workspace;
+  float* part_ml = part_o + (size_t)B * H * nsplit * HD;
+  int rc;
+  if ((rc = decode_attn_partials(what, qkv, cache, part_o, part_ml, pos, pos_stride, B, H, max_seqlen, nsplit, softmax_scale, stream))) return rc;
   EVO_CUDA(launch_pdl(decode_attn_merge_kernel, dim3(H, B), dim3(HD), 0, (cudaStream_t)stream, (const float*)part_o, (const float*)part_ml, (bf16*)out, H, nsplit));
   return check_launch("evo_decode_attn_merge");
 }
@@ -353,4 +578,62 @@ extern "C" int evo_advance_positions(int64_t* pos, int B, int64_t delta, void* s
   EVO_REQUIRE(B >= 1, "evo_advance_positions: bad batch %d", B);
   EVO_CUDA(launch_pdl(add_i64_rows_kernel, dim3((B + 127) / 128), dim3(128), 0, (cudaStream_t)stream, (long long*)pos, B, (long long)delta));
   return check_launch("evo_advance_positions");
+}
+
+extern "C" int evo_decode_qkv_prep_shared(void* qkv, void* suffix_cache, const void* cos, const void* sin, const int64_t* pos, const int64_t* spos,
+                                          int B, int H, int hd, int64_t suffix_len, void* stream) {
+  EVO_REQUIRE(hd == HD, "evo_decode_qkv_prep_shared: head_dim %d unsupported", hd);
+  EVO_REQUIRE(B >= 1 && H >= 1 && suffix_len >= 1, "evo_decode_qkv_prep_shared: bad batch %d, heads %d or suffix length %lld", B, H, (long long)suffix_len);
+  int n = B * H * 64;
+  EVO_CUDA(launch_pdl(decode_qkv_prep_shared_kernel, dim3((n + 127) / 128), dim3(128), 0, (cudaStream_t)stream, (bf16*)qkv, (bf16*)suffix_cache,
+                      (const bf16*)cos, (const bf16*)sin, (const long long*)pos, (const long long*)spos, B, H, (long long)suffix_len));
+  return check_launch("evo_decode_qkv_prep_shared");
+}
+
+extern "C" size_t evo_decode_attn_shared_workspace(int B, int H, int nsplit_prefix, int nsplit_suffix) {
+  return (size_t)B * H * (nsplit_prefix + nsplit_suffix) * (HD + 2) * sizeof(float);
+}
+
+extern "C" int evo_decode_attn_shared(const void* qkv, const void* prefix_cache, const int64_t* group_offsets, const int64_t* prefix_len, int G,
+                                      int64_t prefix_cache_len, const void* suffix_cache, const int64_t* spos, int64_t suffix_len, void* out,
+                                      int B, int H, int hd, int nsplit_prefix, int nsplit_suffix, float softmax_scale,
+                                      void* workspace, size_t workspace_bytes, void* stream) {
+  const char* what = "evo_decode_attn_shared";
+  EVO_REQUIRE(hd == HD, "%s: head_dim %d unsupported", what, hd);
+  EVO_REQUIRE(B >= 1 && G >= 1 && G <= B && H >= 1 && H <= 65535, "%s: bad batch %d, group count %d or head count %d", what, B, G, H);
+  EVO_REQUIRE(nsplit_prefix >= 1 && nsplit_prefix <= 64 && nsplit_suffix >= 1 && nsplit_suffix <= 64, "%s: bad nsplit %d / %d", what, nsplit_prefix, nsplit_suffix);
+  EVO_REQUIRE(prefix_cache_len >= 1 && (long long)G * prefix_cache_len < (1LL << 31) && suffix_len >= 1,
+              "%s: bad cache lengths (prefix %lld x %d groups, suffix %lld)", what, (long long)prefix_cache_len, G, (long long)suffix_len);
+  EVO_REQUIRE(group_offsets && prefix_len && spos, "%s: needs group_offsets, prefix_len and spos", what);
+  EVO_REQUIRE(workspace && workspace_bytes >= evo_decode_attn_shared_workspace(B, H, nsplit_prefix, nsplit_suffix), "%s: workspace too small", what);
+  float* pre_o = (float*)workspace;
+  float* pre_ml = pre_o + (size_t)B * H * nsplit_prefix * HD;
+  float* suf_o = pre_ml + (size_t)B * H * nsplit_prefix * 2;
+  float* suf_ml = suf_o + (size_t)B * H * nsplit_suffix * HD;
+  cudaStream_t st = (cudaStream_t)stream;
+  int rc;
+  CUtensorMap tmQ, tmKV;
+  {
+    const uint64_t dims[3] = {(uint64_t)HD, (uint64_t)H, (uint64_t)B};                 // q of qkv (B, 3, H, 128)
+    const uint64_t str[2] = {(uint64_t)HD * 2, (uint64_t)3 * H * HD * 2};
+    const uint32_t box[3] = {64, 1, (uint32_t)SP_ROWS};
+    if ((rc = make_tmap_nd_bf16(&tmQ, qkv, 3, dims, str, box, true))) return rc;
+  }
+  {
+    const uint64_t dims[3] = {(uint64_t)HD, (uint64_t)(2 * H), (uint64_t)G * (uint64_t)prefix_cache_len};   // (G * P, 2H, 128)
+    const uint64_t str[2] = {(uint64_t)HD * 2, (uint64_t)2 * H * HD * 2};
+    const uint32_t box[3] = {64, 1, (uint32_t)SP_KEYS};
+    if ((rc = make_tmap_nd_bf16(&tmKV, prefix_cache, 3, dims, str, box, true))) return rc;
+  }
+  static unsigned long long attr_done = 0;
+  if ((rc = ensure_dyn_smem(decode_attn_prefix_kernel, SP_SMEM, attr_done))) return rc;
+  // every group has ceil(rows / 64) chunks, so G + B / 64 bounds their number; CTAs past the last chunk exit at once
+  EVO_CUDA(launch_pdl(decode_attn_prefix_kernel, dim3(H, G + B / SP_ROWS, nsplit_prefix), dim3(160), (size_t)SP_SMEM, st, tmQ, tmKV,
+                      (const long long*)group_offsets, (const long long*)prefix_len, G, (long long)prefix_cache_len, B, H, nsplit_prefix,
+                      softmax_scale * 1.4426950408889634f, pre_o, pre_ml));
+  if ((rc = check_launch(what))) return rc;
+  if ((rc = decode_attn_partials(what, qkv, suffix_cache, suf_o, suf_ml, spos, 1, B, H, suffix_len, nsplit_suffix, softmax_scale, stream))) return rc;
+  EVO_CUDA(launch_pdl(decode_attn_merge2_kernel, dim3(H, B), dim3(HD), 0, st, (const float*)pre_o, (const float*)pre_ml, nsplit_prefix,
+                      (const float*)suf_o, (const float*)suf_ml, nsplit_suffix, (bf16*)out, H));
+  return check_launch("evo_decode_attn_shared_merge");
 }

@@ -105,6 +105,40 @@ def ragged_batches(lengths: Sequence[int], n_new: int, batch_size: int = 64, ali
     return out
 
 
+def shared_batches(prompts: Sequence, n_new: int, batch_size: int = 64, align: int = 64):
+    """Plan of shared-prompt generation: (groups, batches).  groups[g] = the input indices of distinct prompt g (identical
+    prompts, strings or token sequences, form one group), in first-seen order.  batches = [(parts, prefill, suffix_len)] per
+    decode batch: parts = [(g, input indices)] with each group's rows contiguous and at most `batch_size` rows in all, groups
+    in order, so a large group continues into the next batch(es); prefill = the groups whose rows first appear in this batch
+    (each prompt is prefilled once, before its first batch, and its prefix lives until its last); suffix_len = the generated
+    tokens' cache length, n_new rounded up to `align`."""
+    if batch_size < 1:
+        raise ValueError("batch_size must be >= 1")
+    index: Dict = {}
+    for i, p in enumerate(prompts):
+        index.setdefault(p if isinstance(p, str) else tuple(p), []).append(i)
+    groups = list(index.values())
+    cut, cur, n = [], [], 0
+    for g, idx in enumerate(groups):
+        k = 0
+        while k < len(idx):
+            take = min(batch_size - n, len(idx) - k)
+            cur.append((g, idx[k:k + take]))
+            n, k = n + take, k + take
+            if n == batch_size:
+                cut.append(cur)
+                cur, n = [], 0
+    if cur:
+        cut.append(cur)
+    suffix_len = (n_new + align - 1) // align * align
+    batches, seen = [], set()
+    for parts in cut:
+        fresh = [g for g, _ in parts if g not in seen]
+        seen.update(fresh)
+        batches.append((parts, fresh, suffix_len))
+    return groups, batches
+
+
 def packs(lengths: Sequence[int], max_tokens: int, bos: int = 1) -> List[Tuple[List[int], List[int]]]:
     """Plan of packed forwards: [(row indices, cu_seqlens)].  Sequences are taken longest first and cut into packs of at most
     `max_tokens` tokens, `bos` extra token per sequence included; inside a pack they stay longest first, so the longest

@@ -183,12 +183,9 @@ class Generator:
         return picked[:, :done], kept_logits[:, :done], state
 
 
-def _generate_ragged(prompt_seqs, model, tokenizer, engine, n_tokens, prepend_bos, batch_size, verbose, packed_prefill=False):
-    """generate(ragged=True): prompts sorted by length and cut into batches of <= batch_size; per batch one ragged prefill
-    (StripedHyena.prefill_ragged), one first pick (evo_sample) and one on-device loop with per-row positions.  Texts and
-    scores come back in input order."""
+def _ragged_ids(prompt_seqs, model, tokenizer, n_tokens, prepend_bos):
+    """The checks of ragged generation, all before anything is launched; returns (token ids per prompt, device)."""
     from . import _lib
-    from .frontend import ragged_batches
     if n_tokens < 1:
         raise ValueError("ragged generation needs n_tokens >= 1")
     if not hasattr(model, "prefill_ragged"):
@@ -203,37 +200,86 @@ def _generate_ragged(prompt_seqs, model, tokenizer, engine, n_tokens, prepend_bo
     too_long = [i for i, t in enumerate(ids) if len(t) > limit]
     if too_long:
         raise _lib.EvoError(f"prompt {too_long[0]} has {len(ids[too_long[0]])} tokens, above the model's max_seqlen {limit}")
-    dev = p0.device
-    V = tokenizer.vocab_size
+    return ids, p0.device
+
+
+def _decode_batch(model, engine, tokenizer, head, state, starts, n_tokens):
+    """First pick from the prefill's head logits, then n_tokens - 1 steps of the on-device loop at per-row positions `starts`;
+    returns (texts, mean log-likelihood scores) of the batch's rows, scored with the reference's alignment (Q3)."""
+    dev = head.device
+    picked = torch.empty(head.shape[0], n_tokens, dtype=torch.long, device=dev)
+    kept_logits = torch.empty(head.shape[0], n_tokens, tokenizer.vocab_size, dtype=torch.float, device=dev)
+    token = engine._pick_device(head)
+    kept_logits[:, 0], picked[:, 0] = head, token
+    if n_tokens > 1:
+        got, got_logits = model.decode_loop(token, state, n_tokens - 1, starts, n_out=n_tokens - 1,
+                                            top_k=engine.top_k, top_p=engine.top_p, temperature=engine.temperature)
+        picked[:, 1:], kept_logits[:, 1:] = got, got_logits
+    decoded = tokenizer.detokenize_batch(picked)
+    # logits_to_logprobs(trim_bos=True) pairs logits[i] with token[i+1]: the reference's alignment (Q3)
+    per_token = logits_to_logprobs(kept_logits, picked).float().cpu().numpy()
+    return decoded, [float(np.mean(row)) for row in per_token]
+
+
+def _generate_shared(prompt_seqs, model, tokenizer, engine, n_tokens, prepend_bos, batch_size, verbose):
+    """generate(ragged=True, share_prompts=True): identical prompts form one group; each distinct prompt is prefilled once
+    (StripedHyena.prefill_prefixes, packed) and its rows decode against its K,V as one shared prefix
+    (StripedHyena.shared_decode_state + decode_loop), in batches of <= batch_size rows (frontend.shared_batches).  Texts and
+    scores come back in input order."""
+    from .frontend import shared_batches
+    ids, _ = _ragged_ids(prompt_seqs, model, tokenizer, n_tokens, prepend_bos)
+    groups, plan = shared_batches(ids, n_tokens, batch_size)
+    last_batch = {g: k for k, (parts, _, _) in enumerate(plan) for g, _ in parts}
+    live = {}                                     # group -> (its prefill's prefixes, its index there), until its last batch
     texts: List[str] = [""] * len(ids)
     scores: List[float] = [0.0] * len(ids)
-    pick_args = dict(top_k=engine.top_k, top_p=engine.top_p, temperature=engine.temperature)
+    for k, (parts, fresh, suffix_len) in enumerate(plan):
+        with torch.inference_mode():
+            if fresh:
+                pre = model.prefill_prefixes([ids[groups[g][0]] for g in fresh])
+                live.update((g, (pre, j)) for j, g in enumerate(fresh))
+                del pre
+            head, state = model.shared_decode_state([live[g] + (len(rows),) for g, rows in parts], suffix_len)
+        for g, _ in parts:
+            if last_batch[g] == k:
+                del live[g]
+        rows = [r for _, rr in parts for r in rr]
+        starts = torch.tensor([len(ids[r]) for r in rows], dtype=torch.int64)
+        decoded, got = _decode_batch(model, engine, tokenizer, head, state, starts, n_tokens)
+        del state, head
+        if verbose > 1:
+            print(f"[generate] shared-prompt batch of {len(rows)} rows in {len(parts)} groups, {len(fresh)} prefilled")
+        for j, r in enumerate(rows):
+            texts[r], scores[r] = decoded[j], got[j]
+    return texts, scores
+
+
+def _generate_ragged(prompt_seqs, model, tokenizer, engine, n_tokens, prepend_bos, batch_size, verbose, packed_prefill=False):
+    """generate(ragged=True): prompts sorted by length and cut into batches of <= batch_size; per batch one ragged prefill
+    (StripedHyena.prefill_ragged), one first pick (evo_sample) and one on-device loop with per-row positions.  Texts and
+    scores come back in input order."""
+    from .frontend import ragged_batches
+    ids, _ = _ragged_ids(prompt_seqs, model, tokenizer, n_tokens, prepend_bos)
+    texts: List[str] = [""] * len(ids)
+    scores: List[float] = [0.0] * len(ids)
     for rows, cache_len in ragged_batches([len(t) for t in ids], n_tokens, batch_size):
-        picked = torch.empty(len(rows), n_tokens, dtype=torch.long, device=dev)
-        kept_logits = torch.empty(len(rows), n_tokens, V, dtype=torch.float, device=dev)
         with torch.inference_mode():
             head, state = model.prefill_ragged([ids[r] for r in rows], cache_len, packed=packed_prefill)
-        token = engine._pick_device(head)
-        kept_logits[:, 0], picked[:, 0] = head, token
-        if n_tokens > 1:
-            start = torch.tensor([len(ids[r]) for r in rows], dtype=torch.int64)
-            got, got_logits = model.decode_loop(token, state, n_tokens - 1, start, n_out=n_tokens - 1, **pick_args)
-            picked[:, 1:], kept_logits[:, 1:] = got, got_logits
+        starts = torch.tensor([len(ids[r]) for r in rows], dtype=torch.int64)
+        decoded, got = _decode_batch(model, engine, tokenizer, head, state, starts, n_tokens)
         del state, head
         if verbose > 1:
             print(f"[generate] ragged batch of {len(rows)}: prompt lengths {len(ids[rows[0]])}..{len(ids[rows[-1]])}, cache {cache_len}")
-        decoded = tokenizer.detokenize_batch(picked)
-        # logits_to_logprobs(trim_bos=True) pairs logits[i] with token[i+1]: the reference's alignment (Q3)
-        per_token = logits_to_logprobs(kept_logits, picked).float().cpu().numpy()
         for k, r in enumerate(rows):
-            texts[r], scores[r] = decoded[k], float(np.mean(per_token[k]))
+            texts[r], scores[r] = decoded[k], got[k]
     return texts, scores
 
 
 def generate(prompt_seqs: List[str], model, tokenizer: CharLevelTokenizer, n_tokens: int = 100, temperature: float = 0.0,
              top_k: int = 1, top_p: float = 1.0, batched: bool = True, prepend_bos: bool = False,
              cached_generation: bool = False, force_prompt_threshold: int = 128, verbose: int = 1,
-             device: str = "cuda:0", ragged: bool = False, batch_size: int = 64, packed_prefill: bool = False, **kwargs) -> Tuple[List[str], List[float]]:
+             device: str = "cuda:0", ragged: bool = False, batch_size: int = 64, packed_prefill: bool = False, share_prompts: bool = False,
+             **kwargs) -> Tuple[List[str], List[float]]:
     """Sequences and mean log-likelihood "scores" for a list of prompts.  Prompts of one common
     length run as one batch; anything else falls back to one prompt at a time (with a note on stderr).
 
@@ -243,16 +289,26 @@ def generate(prompt_seqs: List[str], model, tokenizer: CharLevelTokenizer, n_tok
     jump to the full prompt length (Q1) never happens.  Needs cached_generation=True, a CUDA model, non-empty prompts no
     longer than the model's max_seqlen, and n_tokens >= 1; texts and scores come back in input order.  packed_prefill=True
     prefills each batch with one packed forward (StripedHyena.prefill_ragged(packed=True)) instead of one forward per
-    distinct prompt length."""
+    distinct prompt length.
+
+    share_prompts=True (with ragged=True) draws many samples of a prompt from one prefill: identical prompts form a group,
+    each distinct prompt is prefilled once per call, and the group's rows decode against its K,V as one shared prefix
+    instead of holding and re-reading a copy each (frontend.shared_batches keeps a group's rows contiguous in batches of at
+    most `batch_size` rows).  Texts and scores come back in input order, scored as with ragged=True."""
     model.eval()
     engine = Generator(model, tokenizer, top_k=top_k, top_p=top_p, temperature=temperature)
+    if share_prompts and not ragged:
+        raise ValueError("share_prompts=True needs ragged=True")
     if ragged:
         if not cached_generation:
             raise ValueError("ragged generation needs cached_generation=True")
         if batch_size < 1:
             raise ValueError("batch_size must be >= 1")
-        texts, scores = _generate_ragged(list(prompt_seqs), model, tokenizer, engine, int(n_tokens), prepend_bos, int(batch_size), verbose,
-                                         packed_prefill=bool(packed_prefill))
+        if share_prompts:
+            texts, scores = _generate_shared(list(prompt_seqs), model, tokenizer, engine, int(n_tokens), prepend_bos, int(batch_size), verbose)
+        else:
+            texts, scores = _generate_ragged(list(prompt_seqs), model, tokenizer, engine, int(n_tokens), prepend_bos, int(batch_size), verbose,
+                                             packed_prefill=bool(packed_prefill))
         if verbose:
             for prompt, text, score in zip(prompt_seqs, texts, scores):
                 print(f'Prompt: "{prompt}",\tOutput: "{text}",\tScore: {score}')

@@ -9,13 +9,20 @@ from torch import Tensor
 @dataclass
 class InferenceParams:
     """Attention side: KV cache per layer, (max_batch, max_seqlen, 2, heads, head_dim) bf16
-    (flash_attn/modules/mha.py:344-370 layout)."""
+    (flash_attn/modules/mha.py:344-370 layout).
+
+    Shared-prompt decoding (StripedHyena.prefill_shared) adds one prefix per group of rows that sample the same prompt:
+    prefix_key_value_memory_dict[layer] (G, P, 2, heads, head_dim) bf16, group_offsets (G + 1) int64 row offsets and
+    prefix_len (G) int64 prompt lengths, both on the device; key_value_memory_dict then holds each row's generated tokens only."""
     max_seqlen: int
     max_batch_size: int
     seqlen_offset: int = 0
     batch_size_offset: int = 0
     key_value_memory_dict: dict = field(default_factory=dict)
     lengths_per_sample: Optional[Tensor] = None
+    prefix_key_value_memory_dict: Optional[dict] = None
+    group_offsets: Optional[Tensor] = None
+    prefix_len: Optional[Tensor] = None
 
     def reset(self, max_seqlen, max_batch_size):
         self.max_seqlen = max_seqlen

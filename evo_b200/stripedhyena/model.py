@@ -708,17 +708,19 @@ class StripedHyena(nn.Module):
         self._tiled = t
         return t
 
-    def _decode_body(self, x, pos_dev, ipd, B, per_row=False):
+    def _decode_body(self, x, pos_dev, ipd, B, per_row=False, shared=None):
         """One token per sequence through all blocks; every launch reads the position from pos_dev: one shared int64, or
-        (per_row) one per row, pos_dev[b] for row b (the _rows entry points)."""
+        (per_row) one per row, pos_dev[b] for row b (the _rows entry points).  shared (a shared-prompt state, see
+        prefill_shared): {"spos": (B,) suffix positions on the device, "chunks": 64-row chunks of the groups}; the _shared entry
+        points then read each group's prefix once and append to the rows' suffix caches."""
         lib = _lib.lib()
         prev = lib.evo_set_pdl(int(self.decode_pdl))
         try:
-            return self._decode_body_impl(x, pos_dev, ipd, B, per_row)
+            return self._decode_body_impl(x, pos_dev, ipd, B, per_row, shared)
         finally:
             lib.evo_set_pdl(prev)
 
-    def _decode_body_impl(self, x, pos_dev, ipd, B, per_row=False):
+    def _decode_body_impl(self, x, pos_dev, ipd, B, per_row=False, shared=None):
         cfg = self.config
         d, H, V = cfg.hidden_size, cfg.num_attention_heads, cfg.vocab_size
         hd = d // H
@@ -740,7 +742,8 @@ class StripedHyena(nn.Module):
 
         u = torch.empty(B, d, dtype=torch.bfloat16, device=dev)
         check(lib.evo_embed(ptr(x), int(x.dtype == torch.int64), ptr(self.embedding_layer.weight), ptr(u), B, d, V, self._stream()), "evo_embed")
-        nsplit = max(1, min(16, -(-8 * torch.cuda.get_device_properties(dev).multi_processor_count // (H * B))))   # >= ~4 waves of 2 CTAs/SM
+        n_sm = torch.cuda.get_device_properties(dev).multi_processor_count
+        nsplit = max(1, min(16, -(-8 * n_sm // (H * B))))   # >= ~4 waves of 2 CTAs/SM
         for i, blk in enumerate(self.blocks):
             xn = torch.empty_like(u)
             self._rmsnorm(u, blk.pre_norm.scale, xn, B)
@@ -750,13 +753,16 @@ class StripedHyena(nn.Module):
                 qkv = torch.empty(B, 3 * d, dtype=torch.bfloat16, device=dev)
                 lin(xn, wsel(i, "in", mha.Wqkv.weight), qkv, 3 * d, d, EPI_BIAS if mha.Wqkv.bias is not None else EPI_NONE, bias=mha.Wqkv.bias)
                 cache = mha_ip.key_value_memory_dict[i]
-                cos, sin = self._rope_tables(cache.shape[1], dev)
-                check(qkv_prep(ptr(qkv), ptr(cache), ptr(cos), ptr(sin), ptr(pos_dev), B, H, hd, cache.shape[1], self._stream()), "evo_decode_qkv_prep")
-                nws = lib.evo_decode_attn_workspace(B, H, nsplit)
-                ws = torch.empty(nws, dtype=torch.uint8, device=dev)
                 ctx = xn
-                check(decode_attn(ptr(qkv), ptr(cache), ptr(ctx), ptr(pos_dev), B, H, hd, cache.shape[1], nsplit,
-                                          1.0 / math.sqrt(hd), ptr(ws), nws, self._stream()), "evo_decode_attn")
+                if shared is not None:
+                    self._decode_attn_shared(i, qkv, ctx, pos_dev, shared, mha_ip, B, n_sm, nsplit)
+                else:
+                    cos, sin = self._rope_tables(cache.shape[1], dev)
+                    check(qkv_prep(ptr(qkv), ptr(cache), ptr(cos), ptr(sin), ptr(pos_dev), B, H, hd, cache.shape[1], self._stream()), "evo_decode_qkv_prep")
+                    nws = lib.evo_decode_attn_workspace(B, H, nsplit)
+                    ws = torch.empty(nws, dtype=torch.uint8, device=dev)
+                    check(decode_attn(ptr(qkv), ptr(cache), ptr(ctx), ptr(pos_dev), B, H, hd, cache.shape[1], nsplit,
+                                              1.0 / math.sqrt(hd), ptr(ws), nws, self._stream()), "evo_decode_attn")
                 lin(ctx, wsel(i, "out", mha.out_proj.weight), u2, d, d, EPI_BIAS_RESID if mha.out_proj.bias is not None else EPI_RESID,
                     bias=mha.out_proj.bias, resid=u)
             else:
@@ -793,6 +799,26 @@ class StripedHyena(nn.Module):
         logits = torch.empty(B, V, dtype=torch.bfloat16, device=dev)
         lin(u, tiled["unembed"] if tiled is not None else self.unembed.weight, logits, V, d, EPI_NONE)
         return logits
+
+    def _decode_attn_shared(self, i, qkv, ctx, pos_dev, shared, mha_ip, B, n_sm, nsplit):
+        """Attention of one decode step of a shared-prompt batch: rotary at pos[b], k,v appended at the row's suffix position,
+        then one query per row over its group's prefix (read once per 64-row chunk) and its own suffix."""
+        H = self.config.num_attention_heads
+        hd = self.config.hidden_size // H
+        lib, dev = _lib.lib(), qkv.device
+        cache, pcache = mha_ip.key_value_memory_dict[i], mha_ip.prefix_key_value_memory_dict[i]
+        S, P, G = cache.shape[1], pcache.shape[1], pcache.shape[0]
+        cos, sin = self._rope_tables(P + S, dev)
+        spos = shared["spos"]
+        check(lib.evo_decode_qkv_prep_shared(ptr(qkv), ptr(cache), ptr(cos), ptr(sin), ptr(pos_dev), ptr(spos), B, H, hd, S, self._stream()),
+              "evo_decode_qkv_prep_shared")
+        # prefix: one wave of single-CTA-per-SM blocks, at least two 128-key tiles per split; suffix: no split past its 64-key tiles
+        nsp_p = max(1, min(64, n_sm // (H * shared["chunks"]), -(-P // 256)))
+        nsp_s = max(1, min(nsplit, -(-S // 64)))
+        nws = lib.evo_decode_attn_shared_workspace(B, H, nsp_p, nsp_s)
+        ws = torch.empty(nws, dtype=torch.uint8, device=dev)
+        check(lib.evo_decode_attn_shared(ptr(qkv), ptr(pcache), ptr(mha_ip.group_offsets), ptr(mha_ip.prefix_len), G, P, ptr(cache), ptr(spos), S,
+                                         ptr(ctx), B, H, hd, nsp_p, nsp_s, 1.0 / math.sqrt(hd), ptr(ws), nws, self._stream()), "evo_decode_attn_shared")
 
     # ---- prefill of prompts of different lengths into one decode batch ------------------------------------------------
     def prefill_ragged(self, prompts, cache_len, packed=False):
@@ -872,6 +898,71 @@ class StripedHyena(nn.Module):
             self._gemm(last, self.unembed.weight, head, B, V, d, EPI_NONE)      # the full-logits unembed's variant: the same bits per row
         return head, {"mha": mha, "hyena": hy}
 
+    # ---- shared-prompt sampling: many rows decode from one prefill of their prompt -----------------------------------
+    def prefill_shared(self, prompts, rows_per_prompt, n_new):
+        """Prefill G distinct prompts once and set up a decode batch in which prompt g has rows_per_prompt[g] contiguous rows
+        (a group) that share its K,V as one prefix.  Returns (head (B, V) bf16: each row's logits at its prompt's last
+        position, the inference params dict) with B = sum(rows_per_prompt); decode_loop steps it at start_pos = each row's
+        prompt length.  The attention holder carries the (G, P, 2, H, 128) prefix caches (P = the longest prompt rounded up
+        to 64), group_offsets and prefix_len; its key_value_memory_dict holds (B, round_up(n_new, 64), 2, H, 128) caches for
+        the generated tokens.  Every row gets its own contiguous copy of its group's Hyena states."""
+        if len(rows_per_prompt) != len(prompts):
+            raise ValueError("prefill_shared: one row count per prompt")
+        pre = self.prefill_prefixes(prompts)
+        return self.shared_decode_state([(pre, g, n) for g, n in enumerate(rows_per_prompt)], n_new)
+
+    def prefill_prefixes(self, prompts):
+        """One packed prefill (prefill_ragged(packed=True)) of G distinct non-empty prompts: a dict of their head logits
+        (G, V), (G, P, 2, H, 128) KV caches, Hyena end states and lengths, for shared_decode_state."""
+        lengths = [len(p) for p in prompts]
+        if not lengths or min(lengths) == 0:
+            raise ValueError("prefill_prefixes needs at least one prompt and no empty prompt")
+        head, ipd = self._prefill_packed(prompts, lengths, _round_up(max(lengths), 64))
+        hy = ipd["hyena"]
+        return {"head": head, "caches": ipd["mha"].key_value_memory_dict, "state": hy.state_dict, "fir": hy.fir_state_dict, "lengths": lengths}
+
+    def shared_decode_state(self, parts, n_new):
+        """Decode state of one shared-prompt batch: parts = [(prefix from prefill_prefixes, group index in it, rows)], one group
+        per entry in row order.  Groups that are consecutive in one prefix keep its caches as a view; otherwise their prefix
+        rows are copied into one (G, P, 2, H, 128) cache.  Returns (head (B, V), inference params dict) like prefill_shared."""
+        if not parts or min(n for _, _, n in parts) < 1 or n_new < 1:
+            raise ValueError("shared_decode_state needs at least one group, every group at least one row, and n_new >= 1")
+        cfg = self.config
+        d, H = cfg.hidden_size, cfg.num_attention_heads
+        dev = self.embedding_layer.weight.device
+        counts = [n for _, _, n in parts]
+        B, G = sum(counts), len(parts)
+        plen = [pre["lengths"][g] for pre, g, _ in parts]
+        P = _round_up(max(plen), 64)
+        pre0, g0 = parts[0][0], parts[0][1]
+        as_view = all(pre is pre0 and g == g0 + k for k, (pre, g, _) in enumerate(parts))
+
+        def per_row(get):                        # each group's (1, ...) slice repeated over its rows: one new contiguous tensor
+            return torch.cat([get(pre)[g:g + 1].expand(n, *get(pre).shape[1:]) for pre, g, n in parts]).contiguous()
+
+        with torch.cuda.device(dev), torch.no_grad():
+            prefix = {}
+            for i in sorted(self._attn_idxs):
+                if as_view:
+                    prefix[i] = pre0["caches"][i][g0:g0 + G]
+                else:
+                    prefix[i] = torch.zeros(G, P, 2, H, d // H, dtype=torch.bfloat16, device=dev)
+                    for k, (pre, g, _) in enumerate(parts):
+                        prefix[i][k, :plen[k]] = pre["caches"][i][g, :plen[k]]
+            hy = RecurrentInferenceParams(fir_filter_length=cfg.short_filter_length, state_dim=cfg.state_size, seqlen_offset=0)
+            for i in pre0["state"]:
+                hy.state_dict[i] = per_row(lambda pre: pre["state"][i])
+                hy.fir_state_dict[i] = per_row(lambda pre: pre["fir"][i])
+            head = per_row(lambda pre: pre["head"])
+            S = _round_up(n_new, 64)
+            suffix = {i: torch.zeros(B, S, 2, H, d // H, dtype=torch.bfloat16, device=dev) for i in sorted(self._attn_idxs)}
+            offs = torch.tensor([0] + counts, dtype=torch.int64).cumsum_(0)
+            rows_len = torch.tensor(plen, dtype=torch.int64).repeat_interleave(torch.tensor(counts))
+            mha = InferenceParams(max_seqlen=S, max_batch_size=B, seqlen_offset=0, key_value_memory_dict=suffix,
+                                  lengths_per_sample=rows_len.to(dev), prefix_key_value_memory_dict=prefix,
+                                  group_offsets=offs.to(dev), prefix_len=torch.tensor(plen, dtype=torch.int64, device=dev))
+        return head, {"mha": mha, "hyena": hy}
+
     # ---- on-device generation loop (SURVEY 8f-2): token pick + bookkeeping + feedback inside the captured step ------
     def decode_loop(self, first_token, ipd, n_steps, start_pos, *, top_k=1, top_p=0.0, temperature=1.0, forced=None, n_out=None, seed=None):
         """Run `n_steps` single-token steps without returning to the host in between.
@@ -907,9 +998,19 @@ class StripedHyena(nn.Module):
             last = int(starts.max())
         else:
             last = start_pos = int(start_pos)
+        shared = None
+        if mha_ip.prefix_len is not None:      # shared-prompt state (prefill_shared): the suffix caches hold the generated tokens only
+            if not per_row:
+                raise ValueError("a shared-prompt state needs per-row start positions (each row's prompt length)")
+            counts = torch.diff(mha_ip.group_offsets.cpu())
+            sstarts = starts - mha_ip.prefix_len.cpu().repeat_interleave(counts)
+            if int(sstarts.min()) < 0:
+                raise ValueError("a start position lies inside its row's shared prompt")
+            shared = {"chunks": int(((counts + 63) // 64).sum())}
+        fill = last if shared is None else int(sstarts.max())     # the last cache row a step writes is fill + n_steps - 1
         for i in mha_ip.key_value_memory_dict:
-            if last + n_steps > mha_ip.key_value_memory_dict[i].shape[1]:
-                raise _lib.EvoError(f"sequence length {last + n_steps} exceeds the KV cache ({mha_ip.key_value_memory_dict[i].shape[1]}) (mha.py:367)")
+            if fill + n_steps > mha_ip.key_value_memory_dict[i].shape[1]:
+                raise _lib.EvoError(f"sequence length {fill + n_steps} exceeds the KV cache ({mha_ip.key_value_memory_dict[i].shape[1]}) (mha.py:367)")
         with torch.cuda.device(dev), torch.no_grad():
             self._ensure_packed()
             for i in list(hy_ip.state_dict):
@@ -926,12 +1027,18 @@ class StripedHyena(nn.Module):
             key = ("loop_rows" if per_row else "loop", B, tuple(hy_ip.state_dict[i].data_ptr() for i in sorted(hy_ip.state_dict)),
                    tuple(hy_ip.fir_state_dict[i].data_ptr() for i in sorted(hy_ip.fir_state_dict)),
                    tuple((mha_ip.key_value_memory_dict[i].data_ptr(), mha_ip.key_value_memory_dict[i].shape[1]) for i in sorted(mha_ip.key_value_memory_dict)))
+            if shared is not None:
+                pre = mha_ip.prefix_key_value_memory_dict
+                key = ("loop_shared",) + key[1:] + (tuple((pre[i].data_ptr(), tuple(pre[i].shape)) for i in sorted(pre)),
+                                                    mha_ip.group_offsets.data_ptr(), mha_ip.prefix_len.data_ptr(), shared["chunks"])
             st = self._loop
             if st is None or st["key"] != key:
                 st = {"key": key, "graph": None, "x": torch.empty(B, 1, dtype=torch.long, device=dev),
                       "pos": torch.zeros(B if per_row else 1, dtype=torch.int64, device=dev),
                       "step": torch.zeros(1, dtype=torch.int64, device=dev), "lp": torch.zeros(C.sizeof(_lib.LoopParams), dtype=torch.uint8, device=dev),
                       "lp_host": torch.zeros(C.sizeof(_lib.LoopParams), dtype=torch.uint8).pin_memory()}
+                if shared is not None:
+                    st["spos"] = torch.zeros(B, dtype=torch.int64, device=dev)
                 self._loop = st
             if st.get("lp_copied") is not None:
                 st["lp_copied"].synchronize()       # a previous call's async copy may not have left the pinned staging buffer yet
@@ -941,16 +1048,21 @@ class StripedHyena(nn.Module):
             st["lp_copied"].record()
             if per_row:
                 st["pos"].copy_(starts)
+                if shared is not None:
+                    st["spos"].copy_(sstarts)
+                    shared["spos"] = st["spos"]
             else:
                 st["pos"].fill_(int(start_pos))
             st["step"].zero_()
             st["x"].copy_(x.to(torch.long))
 
             def one_step():
-                logits = self._decode_body(st["x"], st["pos"], ipd, B, per_row)
+                logits = self._decode_body(st["x"], st["pos"], ipd, B, per_row, shared)
                 prev = lib.evo_set_pdl(int(self.decode_pdl))
                 try:
                     check(lib.evo_sample_step(ptr(logits), ptr(st["x"]), B, V, ptr(st["lp"]), ptr(st["step"]), self._stream()), "evo_sample_step")
+                    if shared is not None:
+                        check(lib.evo_advance_positions(ptr(st["spos"]), B, 1, self._stream()), "evo_advance_positions")
                     if per_row:
                         check(lib.evo_advance_positions(ptr(st["pos"]), B, 1, self._stream()), "evo_advance_positions")
                         check(lib.evo_advance_counters(None, ptr(st["step"]), 1, self._stream()), "evo_advance_counters")

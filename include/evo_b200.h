@@ -259,6 +259,28 @@ int evo_decode_qkv_prep_rows(void* qkv, void* cache, const void* cos, const void
 int evo_decode_attn_rows(const void* qkv, const void* cache, void* out, const int64_t* pos, int B, int H, int hd,
                          int64_t max_seqlen, int nsplit, float softmax_scale, void* workspace, size_t workspace_bytes, void* stream);
 int evo_advance_positions(int64_t* pos, int B, int64_t delta, void* stream);
+/* Shared-prompt decode (many samples of one prompt): the B rows form G groups of contiguous rows, group g = rows
+ * [group_offsets[g], group_offsets[g+1]) ((G + 1) int64 DEVICE array, group_offsets[0] = 0, group_offsets[G] = B), and a
+ * group's rows share one prefix of K,V: prefix_cache (G, prefix_cache_len, 2, H, 128) bf16, group g's keys at rows
+ * [0, prefix_len[g]) of its slice (prefix_len: (G) int64 DEVICE array, 1 <= prefix_len[g] <= prefix_cache_len; rows at or past
+ * it may hold anything, NaN included).  Each row's generated tokens live in its own suffix_cache (B, suffix_len, 2, H, 128) bf16.
+ * pos: (B) int64 DEVICE array of absolute positions; spos: (B) int64 DEVICE array of suffix positions,
+ * spos[b] = pos[b] - prefix_len[g(b)].
+ * evo_decode_qkv_prep_shared: rotary on q,k of qkv (B, 3, H, 128) at position pos[b] (evo_decode_qkv_prep_rows' arithmetic)
+ *   and k,v appended at suffix_cache row spos[b].
+ * evo_decode_attn_shared: out (B, H*128) bf16 = one query per row over [prefix keys [0, prefix_len[g(b)]) | suffix keys
+ *   [0, spos[b]]], as three launches: a wgmma kernel that streams each group's prefix once for all its rows (grid (head, 64-row
+ *   chunk of a group, prefix split), nsplit_prefix splits of the prefix), the _rows decode kernel over the suffix cache at
+ *   positions spos (nsplit_suffix splits), and a merge of both partial sets.  fp32 scores and statistics, P rounded to bf16
+ *   before the PV product, one bf16 rounding of the output.  G * prefix_cache_len < 2^31.
+ *   workspace: evo_decode_attn_shared_workspace() bytes. */
+int evo_decode_qkv_prep_shared(void* qkv, void* suffix_cache, const void* cos, const void* sin, const int64_t* pos, const int64_t* spos,
+                               int B, int H, int hd, int64_t suffix_len, void* stream);
+size_t evo_decode_attn_shared_workspace(int B, int H, int nsplit_prefix, int nsplit_suffix);
+int evo_decode_attn_shared(const void* qkv, const void* prefix_cache, const int64_t* group_offsets, const int64_t* prefix_len, int G,
+                           int64_t prefix_cache_len, const void* suffix_cache, const int64_t* spos, int64_t suffix_len, void* out,
+                           int B, int H, int hd, int nsplit_prefix, int nsplit_suffix, float softmax_scale,
+                           void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---- device-side sampler and generation loop: stripedhyena.sample.sample (evo/generation.py:162-167) and the host half
  * of the token loop (evo/generation.py:131-189) ----

@@ -12,8 +12,11 @@ Generates sequences from a prompt with the reference's sampling arguments (scrip
 evo_b200 engine.  With --cached-generation (the default) the token loop runs on the GPU (one CUDA graph per token, device
 sampler); --seed makes a sampled run reproducible.  --prompts-csv reads the prompts from the first column of a CSV with a
 header row (semantic_design's format) and generates them all in batches of up to --batch-size, whatever their lengths
-(ragged generation: the whole prompt is prefilled, one position per row while decoding); outputs come in file order.  The boolean flags keep the reference's `type=bool` parsing (any non-empty
-value is True).
+(ragged generation: the whole prompt is prefilled, one position per row while decoding); outputs come in file order.
+--samples-per-prompt K repeats each CSV prompt K times, prompt-major (semantic_design's n_sample_per_prompt).
+--share-prompts sends the samples of one prompt (--prompt with --n-samples, or repeated CSV prompts) through shared-prompt
+sampling: each distinct prompt is prefilled once and its samples decode against one shared copy of its K,V.  The boolean
+flags keep the reference's `type=bool` parsing (any non-empty value is True).
 """
 import argparse
 
@@ -43,6 +46,9 @@ def build_parser():
     parser.add_argument('--prompts-csv', type=str, default=None,
                         help='CSV whose first column (after a header row) holds the prompts; generates every prompt once, batched whatever their lengths')
     parser.add_argument('--batch-size', type=int, default=64, help='Prompts per decode batch with --prompts-csv')
+    parser.add_argument('--samples-per-prompt', type=int, default=1, help='Samples of each --prompts-csv prompt, prompt-major')
+    parser.add_argument('--share-prompts', action='store_true',
+                        help='Prefill each distinct prompt once and decode its samples against one shared K,V prefix')
     return parser
 
 
@@ -54,10 +60,17 @@ def main(argv=None):
     if args.seed is not None:
         torch.manual_seed(args.seed)
     print('Generated sequences:')
+    if args.samples_per_prompt < 1:
+        raise SystemExit('--samples-per-prompt must be >= 1')
     if args.prompts_csv is not None:
-        return generate(read_prompts_csv(args.prompts_csv), model, tokenizer, n_tokens=args.n_tokens, temperature=args.temperature,
+        prompts = [p for p in read_prompts_csv(args.prompts_csv) for _ in range(args.samples_per_prompt)]
+        return generate(prompts, model, tokenizer, n_tokens=args.n_tokens, temperature=args.temperature,
                         top_k=args.top_k, top_p=args.top_p, cached_generation=True, prepend_bos=args.prepend_bos, device=args.device,
-                        verbose=args.verbose, ragged=True, batch_size=args.batch_size)
+                        verbose=args.verbose, ragged=True, batch_size=args.batch_size, share_prompts=args.share_prompts)
+    if args.share_prompts:
+        return generate([args.prompt] * args.n_samples, model, tokenizer, n_tokens=args.n_tokens, temperature=args.temperature,
+                        top_k=args.top_k, top_p=args.top_p, cached_generation=True, prepend_bos=args.prepend_bos, device=args.device,
+                        verbose=args.verbose, ragged=True, batch_size=args.batch_size, share_prompts=True)
     return generate([args.prompt] * args.n_samples, model, tokenizer, n_tokens=args.n_tokens, temperature=args.temperature,
                     top_k=args.top_k, top_p=args.top_p, cached_generation=args.cached_generation, batched=args.batched,
                     prepend_bos=args.prepend_bos, device=args.device, verbose=args.verbose)
