@@ -11,8 +11,12 @@
 //   The two consumer warpgroups work on the same K / V tiles, so while one runs its softmax the other keeps the
 //   tensor cores busy.
 //
-// Arithmetic matches FlashAttention's: fp32 scores and statistics, P rounded to bf16 for the
-// PV product, fp32 accumulation, single bf16 rounding of the output.
+// Rounding points match FlashAttention's: fp32 scores and statistics, P rounded to bf16 for the
+// PV product, fp32 accumulation, single bf16 rounding of the output.  The running max does not: P
+// is taken against a reference that may lag the row's max by up to 2^8, so P in (1, 2^8] is
+// rounded to bf16 (same relative error as P <= 1), and alpha = ex2(m_ref - mx) flushes to 0 after
+// a jump past 2^126.  tests/test_gpu_attention_peaked.py holds rows with a moving max to the fp64
+// and bf16-oracle bars of the other attention tests, and one-hot and tied rows bit for bit.
 #include "common.cuh"
 #include "wgmma.cuh"
 #include <type_traits>
