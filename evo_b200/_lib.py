@@ -52,6 +52,20 @@ class HyenaVarlenParams(C.Structure):
                 ("state_out", C.c_void_p), ("fir_state_out", C.c_void_p), ("seg_len", C.c_int64)]
 
 
+class HyenaVarlenCkptParams(C.Structure):
+    _fields_ = [("base", HyenaVarlenParams),
+                ("ckpt_states", C.c_void_p), ("ckpt_base", C.c_void_p), ("ckpt_stride", C.c_int64), ("n_ckpt", C.c_int64),
+                ("start_idx", C.c_void_p), ("state_table", C.c_void_p), ("halo_table", C.c_void_p), ("n_table", C.c_int64)]
+
+
+class AttnVarlenPrefixParams(C.Structure):
+    _fields_ = [("qkv", C.c_void_p), ("out", C.c_void_p),
+                ("cu_seqlens", C.c_void_p), ("n_seq", C.c_int), ("T", C.c_int64), ("max_seqlen", C.c_int64),
+                ("cache", C.c_void_p), ("n_cache", C.c_int), ("cache_len", C.c_int64),
+                ("prefix_seq", C.c_void_p), ("prefix_len", C.c_void_p),
+                ("H", C.c_int), ("hd", C.c_int), ("softmax_scale", C.c_float)]
+
+
 class AttnVarlenParams(C.Structure):
     _fields_ = [("q", C.c_void_p), ("k", C.c_void_p), ("v", C.c_void_p), ("out", C.c_void_p),
                 ("q_tok_stride", C.c_int64), ("kv_tok_stride", C.c_int64),
@@ -98,6 +112,8 @@ SIGNATURES = {
     "evo_hyena_fwd": (C.c_int, [C.POINTER(HyenaParams), C.c_void_p, C.c_size_t, C.c_void_p]),
     "evo_hyena_fwd_varlen_workspace": (C.c_size_t, [C.POINTER(HyenaVarlenParams)]),
     "evo_hyena_fwd_varlen": (C.c_int, [C.POINTER(HyenaVarlenParams), C.c_void_p, C.c_size_t, C.c_void_p]),
+    "evo_hyena_fwd_varlen_ckpt_workspace": (C.c_size_t, [C.POINTER(HyenaVarlenCkptParams)]),
+    "evo_hyena_fwd_varlen_ckpt": (C.c_int, [C.POINTER(HyenaVarlenCkptParams), C.c_void_p, C.c_size_t, C.c_void_p]),
     "evo_hyena_step": (C.c_int, [C.c_void_p] * 9 + [C.c_int] * 4 + [C.c_void_p]),
     "evo_hyena_combine_states": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "evo_peer_publish": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
@@ -108,6 +124,7 @@ SIGNATURES = {
     "evo_attn_fwd_ws": (C.c_int, [C.POINTER(AttnParams), C.c_int, C.c_void_p, C.c_size_t, C.c_void_p]),
     "evo_kv_append": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_int64, C.c_int64, C.c_void_p]),
     "evo_attn_fwd_varlen": (C.c_int, [C.POINTER(AttnVarlenParams), C.c_void_p]),
+    "evo_attn_fwd_varlen_prefix": (C.c_int, [C.POINTER(AttnVarlenPrefixParams), C.c_void_p]),
     "evo_kv_append_varlen": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_int64, C.c_int, C.c_int, C.c_int64, C.c_void_p]),
     "evo_gelu_gate_interleaved": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p]),
     "evo_decode_qkv_prep": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int64, C.c_void_p]),

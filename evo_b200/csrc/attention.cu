@@ -48,16 +48,36 @@ struct AttArgsV : AttArgs {      // packed sequences (VARLEN); AttArgs itself st
   const long long* cu_seqlens;   // (B + 1) row offsets; Lq = Lk = the longest length
   long long T;                   // packed rows
 };
+struct AttArgsP : AttArgsV {     // packed queries behind a cached prefix (PREFIX); AttArgsV and its kernels stay as they are
+  const long long* prefix_seq;   // (B) batch row of the cache holding sequence b's prefix
+  const long long* prefix_len;   // (B) prefix keys of sequence b: cache rows [0, prefix_len[b]); its rows sit at positions prefix_len[b] + t
+  long long cache_len;           // rows per batch row of the cache
+  int n_cache;                   // batch rows of the cache
+};
+
+// PREFIX: sequence b's prefix keys, clamped to the cache; 0 in every other form
+template <bool PREFIX, typename A>
+__device__ __forceinline__ long long prefix_keys(const A& a, int b) {
+  if constexpr (PREFIX) return min(max(a.prefix_len[b], 0LL), a.cache_len);
+  else return 0;
+}
 
 __device__ __forceinline__ float ex2(float x) { float y; asm volatile("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 
 // VARLEN: grid row b is packed sequence b = rows [cu[b], cu[b+1]) of (HD, H, T, 1) maps.  Query and key tiles start at the
 // sequence's first row, exactly as in a batch-1 call on it; keys past its end are hidden by the causal mask and query rows past
 // its end are not stored, so the output is that call's bits.
-template <bool VARLEN>
+// PREFIX (implies VARLEN; evo_attn_fwd_varlen_prefix): tmQ maps the packed qkv as (HD, 3H, T, 1) -- q, k, v are heads h, H + h,
+// 2H + h -- and tmK maps a KV cache as (HD, 2H, cache_len, n_cache) -- k, v are heads h, H + h.  Sequence b's rows sit at positions
+// P = prefix_len[b] + t: the key tiles are first the prefix tiles of cache row prefix_seq[b], keys [0, P) from key 0 (no causal
+// mask; keys at or past P masked, and their V rows zeroed in shared memory so that nothing the cache holds there reaches the
+// output), then the sequence's own tiles from its first row, causally.  One online softmax runs over both, so with P % 128 == 0
+// the tiles, masks and bits are those of a batch-1 evo_attn_fwd_ws call with q_pos0 = P on one cache holding both.
+template <bool VARLEN, bool PREFIX = false>
 __global__ void __launch_bounds__(ATT_THREADS, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                const __grid_constant__ CUtensorMap tmV, const std::conditional_t<VARLEN, AttArgsV, AttArgs> a) {
+                const __grid_constant__ CUtensorMap tmV, const std::conditional_t<PREFIX, AttArgsP, std::conditional_t<VARLEN, AttArgsV, AttArgs>> a) {
+  static_assert(!PREFIX || VARLEN, "the prefix form is a packed-sequence form");
   extern __shared__ __align__(1024) uint8_t smem[];            // 128B-swizzled tiles need 1024-byte alignment
   if ((smem_u32(smem) & 1023u) != 0) __trap();               // fail loudly, never compute on a misaligned tile
   uint8_t* sQ = smem;
@@ -84,7 +104,9 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   const long long q0 = (long long)qblk * BQ;
   // keys visible to this block: j <= q_pos0 + q0 + 127, j < Lk
   const long long last_key = min(Lk - 1, a.q_pos0 + q0 + BQ - 1);
-  const int n_kv = (int)(last_key / BKV) + 1;
+  const long long plen = prefix_keys<PREFIX>(a, b);   // PREFIX: prefix keys (0 otherwise) and the tiles that hold them
+  const int n_pre = (int)((plen + BKV - 1) / BKV);
+  const int n_kv = (int)(last_key / BKV) + 1 + n_pre;
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmK); tma_prefetch_desc(&tmV);
@@ -104,6 +126,21 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
       for (int j = 0; j < n_kv; ++j) {
         const int st = j % KV_STAGES;
         const uint32_t ph = (uint32_t)(j / KV_STAGES) & 1;
+        if constexpr (PREFIX) {                // cache tile (k, v = heads h, H + h of tmK) or own tile (k, v = heads H + h, 2H + h of tmQ)
+          const bool pre = j < n_pre;
+          const CUtensorMap* m = pre ? &tmK : &tmQ;
+          const int key0 = pre ? j * BKV : (int)row0 + (j - n_pre) * BKV, kh = pre ? h : a.H + h, vh = kh + a.H;
+          const int zz = pre ? (int)min(max(a.prefix_seq[b], 0LL), (long long)a.n_cache - 1) : 0;
+          mbar_wait(&k_empty[st], ph ^ 1);
+          mbar_arrive_expect_tx(&k_full[st], TILE_BYTES);
+          tma_load_4d(sK + st * TILE_BYTES, m, &k_full[st], 0, kh, key0, zz);
+          tma_load_4d(sK + st * TILE_BYTES + HALF_BYTES, m, &k_full[st], 64, kh, key0, zz);
+          mbar_wait(&v_empty[st], ph ^ 1);
+          mbar_arrive_expect_tx(&v_full[st], TILE_BYTES);
+          tma_load_4d(sV + st * TILE_BYTES, m, &v_full[st], 0, vh, key0, zz);
+          tma_load_4d(sV + st * TILE_BYTES + HALF_BYTES, m, &v_full[st], 64, vh, key0, zz);
+          continue;
+        }
         const int key0 = (int)row0 + j * BKV;
         mbar_wait(&k_empty[st], ph ^ 1);
         mbar_arrive_expect_tx(&k_full[st], TILE_BYTES);
@@ -120,7 +157,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     setmaxnreg_inc<232>();
     const int cw = wg - 1, warp = tid >> 5, lane = tid & 31, quad = lane & 3;
     const int r0 = cw * 64 + warp * 16 + (lane >> 2);        // this thread's rows: r0 and r0 + 8 of the block
-    const long long pos[2] = {a.q_pos0 + q0 + r0, a.q_pos0 + q0 + r0 + 8};
+    const long long pos[2] = {a.q_pos0 + q0 + r0 + plen, a.q_pos0 + q0 + r0 + 8 + plen};
     float o[HD / 2];
     float m_ref[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
 #pragma unroll
@@ -144,14 +181,29 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
       wgmma_fence_regs(s);
       if (lane == 0) mbar_arrive(&k_empty[st]);
       // causal / length mask on tiles that reach past a row's position
-      const long long key0 = (long long)j * BKV + 2 * quad;
+      const bool pre_tile = PREFIX && j < n_pre;
+      if constexpr (PREFIX) {      // a prefix tile's keys run from 0 and stop at plen; own keys run from position plen
+        const long long key0 = (pre_tile ? (long long)j * BKV : plen + (long long)(j - n_pre) * BKV) + 2 * quad;
 #pragma unroll
-      for (int hr = 0; hr < 2; ++hr) {
-        if (key0 + BKV - 1 - 2 * quad > pos[hr]) {
+        for (int hr = 0; hr < 2; ++hr) {
+          const long long lim = pre_tile ? plen - 1 : pos[hr];
+          if (key0 + BKV - 1 - 2 * quad > lim) {
 #pragma unroll
-          for (int i = 0; i < BKV / 8; ++i)
+            for (int i = 0; i < BKV / 8; ++i)
 #pragma unroll
-            for (int e = 0; e < 2; ++e) if (key0 + 8 * i + e > pos[hr]) s[4 * i + 2 * hr + e] = -INFINITY;
+              for (int e = 0; e < 2; ++e) if (key0 + 8 * i + e > lim) s[4 * i + 2 * hr + e] = -INFINITY;
+          }
+        }
+      } else {
+        const long long key0 = (long long)j * BKV + 2 * quad;
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+          if (key0 + BKV - 1 - 2 * quad > pos[hr]) {
+#pragma unroll
+            for (int i = 0; i < BKV / 8; ++i)
+#pragma unroll
+              for (int e = 0; e < 2; ++e) if (key0 + 8 * i + e > pos[hr]) s[4 * i + 2 * hr + e] = -INFINITY;
+          }
         }
       }
       uint32_t pf[BKV / 16][4];                                 // P as the A operand of the PV product, bf16 pairs
@@ -181,6 +233,18 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
         l[hr] += ls;
       }
       mbar_wait(&v_full[st], ph);
+      if constexpr (PREFIX) {
+        if (pre_tile && (long long)(j + 1) * BKV > plen) {   // zero V rows [plen - 128 j, 128): a 128-byte swizzled row stays one row
+          const int nvalid = (int)(plen - (long long)j * BKV);
+          uint8_t* vs = sV + st * TILE_BYTES;
+          for (int idx = threadIdx.x - 128; idx < (BKV - nvalid) * 16; idx += 256) {
+            const int row = nvalid + idx / 16, chunk = idx % 16;
+            *reinterpret_cast<uint4*>(vs + (chunk / 8) * HALF_BYTES + row * 128 + (chunk % 8) * 16) = make_uint4(0, 0, 0, 0);
+          }
+          fence_proxy_async_smem();
+          named_bar_sync(1, 256);
+        }
+      }
       const uint32_t va = smem_u32(sV + st * TILE_BYTES);
       wgmma_fence();
 #pragma unroll
@@ -322,4 +386,38 @@ extern "C" int evo_attn_fwd_varlen(const evo_attn_varlen_params* p, void* stream
   if ((rc = ensure_dyn_smem(attn_fwd_kernel<true>, ATT_SMEM, done))) return rc;
   attn_fwd_kernel<true><<<grid, ATT_THREADS, ATT_SMEM, st>>>(tmQ, tmK, tmV, a);
   return check_launch("evo_attn_fwd_varlen");
+}
+
+extern "C" int evo_attn_fwd_varlen_prefix(const evo_attn_varlen_prefix_params* p, void* stream) {
+  EVO_REQUIRE(p->hd == HD, "evo_attn_fwd_varlen_prefix: head_dim %d unsupported (kernel is specialised for 128)", p->hd);
+  EVO_REQUIRE(p->n_seq > 0 && p->n_seq <= 65535 && p->H > 0 && 3 * p->H <= 65535, "evo_attn_fwd_varlen_prefix: bad sequence count %d or head count %d", p->n_seq, p->H);
+  EVO_REQUIRE(p->cu_seqlens != nullptr && p->max_seqlen > 0 && p->max_seqlen <= p->T && p->T < (1LL << 31),
+              "evo_attn_fwd_varlen_prefix: needs cu_seqlens and 0 < max_seqlen <= T < 2^31 (max_seqlen %lld, T %lld)", (long long)p->max_seqlen, (long long)p->T);
+  EVO_REQUIRE(p->cache != nullptr && p->n_cache > 0 && p->cache_len > 0 && p->cache_len < (1LL << 31) && p->prefix_seq != nullptr && p->prefix_len != nullptr,
+              "evo_attn_fwd_varlen_prefix: needs a cache of n_cache > 0 rows of 0 < cache_len < 2^31 keys, prefix_seq and prefix_len");
+  cudaStream_t st = (cudaStream_t)stream;
+  CUtensorMap tmQKV, tmC;
+  int rc;
+  {
+    uint64_t dims[4] = {(uint64_t)HD, (uint64_t)3 * p->H, (uint64_t)p->T, 1};
+    uint64_t str[3] = {(uint64_t)HD * 2, (uint64_t)3 * p->H * HD * 2, (uint64_t)p->T * 3 * p->H * HD * 2};
+    uint32_t box[4] = {64, 1, BQ, 1};
+    if ((rc = make_tmap_4d(&tmQKV, p->qkv, dims, str, box))) return rc;
+  }
+  {
+    uint64_t dims[4] = {(uint64_t)HD, (uint64_t)2 * p->H, (uint64_t)p->cache_len, (uint64_t)p->n_cache};
+    uint64_t str[3] = {(uint64_t)HD * 2, (uint64_t)2 * p->H * HD * 2, (uint64_t)p->cache_len * 2 * p->H * HD * 2};
+    uint32_t box[4] = {64, 1, BKV, 1};
+    if ((rc = make_tmap_4d(&tmC, p->cache, dims, str, box))) return rc;
+  }
+  AttArgsP a = {};
+  a.out = (bf16*)p->out; a.B = p->n_seq; a.H = p->H; a.Lq = a.Lk = p->max_seqlen; a.q_pos0 = 0;
+  a.scale_log2 = p->softmax_scale * 1.4426950408889634f;
+  a.cu_seqlens = (const long long*)p->cu_seqlens; a.T = p->T;
+  a.prefix_seq = (const long long*)p->prefix_seq; a.prefix_len = (const long long*)p->prefix_len; a.cache_len = p->cache_len; a.n_cache = p->n_cache;
+  dim3 grid((unsigned)((p->max_seqlen + BQ - 1) / BQ), p->H, p->n_seq);
+  static unsigned long long done = 0;
+  if ((rc = ensure_dyn_smem(attn_fwd_kernel<true, true>, ATT_SMEM, done))) return rc;
+  attn_fwd_kernel<true, true><<<grid, ATT_THREADS, ATT_SMEM, st>>>(tmQKV, tmC, tmC, a);
+  return check_launch("evo_attn_fwd_varlen_prefix");
 }

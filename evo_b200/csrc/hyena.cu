@@ -500,6 +500,100 @@ extern "C" int evo_hyena_fwd_varlen(const evo_hyena_varlen_params* p, void* work
   return 0;
 }
 
+// checkpointed / resumed packed sequences: sequence b's last two z rows, with its starting FIR history (halo_table[start_idx[b]])
+// standing in front of row 0 when it is shorter than two rows
+__global__ void fir_state_resume_kernel(const bf16* __restrict__ z, const long long* __restrict__ cu, const long long* __restrict__ start_idx,
+                                        const bf16* __restrict__ halo_table, long long n_table, bf16* __restrict__ out,
+                                        int n_seq, long long T, long long max_len, long long C3) {
+  long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;   // (b, c)
+  if (idx >= (long long)n_seq * C3) return;
+  long long b = idx / C3, c = idx % C3;
+  const long long row0 = min(max(cu[b], 0LL), T);
+  const long long len = min(min(cu[b + 1], T) - row0, max_len);
+  long long sidx = start_idx ? start_idx[b] : -1;
+  if (sidx >= n_table) sidx = -1;
+#pragma unroll
+  for (int k = 0; k < 2; ++k) {
+    long long t = len - 2 + k;
+    bf16 v = __float2bfloat16_rn(0.f);
+    if (t >= 0) v = z[(row0 + t) * C3 + c];
+    else if (sidx >= 0) v = halo_table[(sidx * 2 + (t + 2)) * C3 + c];
+    out[idx * 2 + k] = v;
+  }
+}
+
+// The checkpointed form keeps every segment start on the 16-token stage, so that each checkpoint ends a full tile
+static int ckpt_geometry(const evo_hyena_varlen_ckpt_params* p, int& nseg, long long& seg_len) {
+  int rc;
+  if ((rc = varlen_geometry(&p->base, nseg, seg_len))) return rc;
+  if (p->ckpt_states) {
+    EVO_REQUIRE(p->ckpt_stride > 0 && p->ckpt_stride % 128 == 0 && p->ckpt_base != nullptr && p->n_ckpt > 0,
+                "evo_hyena_fwd_varlen_ckpt: checkpoints need ckpt_base, n_ckpt > 0 and a stride that is a positive multiple of 128 (got %lld)",
+                (long long)p->ckpt_stride);
+    if (p->base.seg_len > 0) {
+      EVO_REQUIRE(seg_len % evo_hy2::T2 == 0, "evo_hyena_fwd_varlen_ckpt: with checkpoints a forced seg_len must be a multiple of %d (got %lld)",
+                  evo_hy2::T2, seg_len);
+    } else {
+      seg_len = (seg_len + evo_hy2::T2 - 1) / evo_hy2::T2 * evo_hy2::T2;
+      nseg = (int)((p->base.max_seqlen + seg_len - 1) / seg_len);
+    }
+  }
+  if (p->start_idx) EVO_REQUIRE(p->state_table != nullptr && p->halo_table != nullptr && p->n_table > 0,
+                                "evo_hyena_fwd_varlen_ckpt: start_idx needs state_table, halo_table and n_table > 0");
+  return 0;
+}
+
+extern "C" size_t evo_hyena_fwd_varlen_ckpt_workspace(const evo_hyena_varlen_ckpt_params* p) {
+  int nseg; long long seg_len;
+  if (ckpt_geometry(p, nseg, seg_len) || nseg <= 1) return 0;
+  return (size_t)p->base.n_seq * nseg * p->base.D * NS * 2 * sizeof(float);
+}
+
+extern "C" int evo_hyena_fwd_varlen_ckpt(const evo_hyena_varlen_ckpt_params* p, void* workspace, size_t workspace_bytes, void* stream) {
+  int nseg; long long seg_len;
+  int rc;
+  if ((rc = ckpt_geometry(p, nseg, seg_len))) return rc;
+  const evo_hyena_varlen_params* q = &p->base;
+  EVO_REQUIRE(q->z != nullptr && q->y != nullptr, "evo_hyena_fwd_varlen_ckpt: z or y is NULL");
+  const size_t need = evo_hyena_fwd_varlen_ckpt_workspace(p);
+  EVO_REQUIRE(workspace_bytes >= need && (need == 0 || workspace), "evo_hyena_fwd_varlen_ckpt: workspace too small (%zu < %zu)", workspace_bytes, need);
+  cudaStream_t st = (cudaStream_t)stream;
+  using namespace evo_hy2;
+  CUtensorMap tmZ;
+  uint64_t dims[3] = {(uint64_t)3 * q->D, (uint64_t)q->T, 1};
+  uint64_t str[2] = {(uint64_t)3 * q->D * 2, (uint64_t)q->T * 3 * q->D * 2};
+  uint32_t box[3] = {128, (uint32_t)T2, 1};
+  if ((rc = make_tmap_nd_bf16(&tmZ, q->z, 3, dims, str, box, false))) return rc;
+  evo_hy3::Args2R a = {};
+  a.y = (bf16*)q->y; a.z = (const bf16*)q->z;
+  a.fir_w = (const bf16*)q->fir_w; a.fir_b = (const bf16*)q->fir_b; a.Dskip = (const bf16*)q->Dskip;
+  a.poles = q->poles; a.residues = q->residues; a.state_out = q->state_out;
+  a.seg_states = (float*)workspace; a.B = q->n_seq; a.D = q->D; a.nseg = nseg; a.L = q->max_seqlen; a.seg_len = seg_len;
+  a.cu_seqlens = (const long long*)q->cu_seqlens; a.T = q->T;
+  a.ckpt_out = p->ckpt_states; a.ckpt_base = (const long long*)p->ckpt_base; a.ckpt_stride = p->ckpt_stride; a.n_ckpt = p->n_ckpt;
+  a.start_idx = (const long long*)p->start_idx; a.state_table = p->state_table; a.halo_table = (const bf16*)p->halo_table; a.n_table = p->n_table;
+  a.nst = 4;
+  static unsigned long long done_s = 0, done_o = 0;
+  if ((rc = ensure_dyn_smem(evo_hy3::hyena_scan_ms_kernel<true, true, true>, smem_bytes(STAGES), done_s))) return rc;
+  if ((rc = ensure_dyn_smem(evo_hy3::hyena_scan_ms_kernel<false, true, true>, smem_bytes(STAGES), done_o))) return rc;
+  const int SMEM_BYTES = smem_bytes(a.nst);
+  dim3 grid(q->D / CH_PER_CTA, q->n_seq, nseg), block(evo_hy3::THREADS);
+  if (nseg > 1) {
+    dim3 g2(grid.x, grid.y, nseg - 1);
+    evo_hy3::hyena_scan_ms_kernel<true, true, true><<<g2, block, SMEM_BYTES, st>>>(tmZ, a);
+    if ((rc = check_launch("hyena_scan_varlen_ckpt<state>"))) return rc;
+  }
+  evo_hy3::hyena_scan_ms_kernel<false, true, true><<<grid, block, SMEM_BYTES, st>>>(tmZ, a);
+  if ((rc = check_launch("hyena_scan_varlen_ckpt<out>"))) return rc;
+  if (q->fir_state_out) {
+    long long n = (long long)q->n_seq * 3 * q->D;
+    fir_state_resume_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>((const bf16*)q->z, (const long long*)q->cu_seqlens, a.start_idx, a.halo_table,
+                                                                         a.n_table, (bf16*)q->fir_state_out, q->n_seq, q->T, q->max_seqlen, 3LL * q->D);
+    if ((rc = check_launch("fir_state_resume"))) return rc;
+  }
+  return 0;
+}
+
 extern "C" int evo_hyena_step(const void* u, void* y, void* fir_state, float* state,
                               const void* fir_w, const void* fir_b, const void* Dskip,
                               const float* poles, const float* residues,

@@ -45,6 +45,13 @@ struct Args2V : Args2 {                      // packed sequences (VARLEN); Args2
   const long long* cu_seqlens;               // (B + 1) row offsets; Args2::L is the longest length
   long long T;                               // packed rows
 };
+struct Args2R : Args2V {                     // checkpoint emission and resumed starts (RESUME); Args2V and its kernels stay as they are
+  // emission: the output pass stores the running state after row k*ckpt_stride - 1 of sequence b at table row ckpt_base[b] + k - 1
+  // (k >= 1, k*ckpt_stride < its length; ckpt_stride a multiple of 128, seg_len a multiple of the 16-token stage), NULL = none
+  float* ckpt_out; const long long* ckpt_base; long long ckpt_stride, n_ckpt;
+  // resumed start: sequence b starts from state_table[start_idx[b]] and FIR history halo_table[start_idx[b]] (-1 = zero start)
+  const long long* start_idx; const float* state_table; const bf16* halo_table; long long n_table;
+};
 
 __device__ __forceinline__ uint32_t mul_bf2(uint32_t a, uint32_t b) { uint32_t d; asm("mul.rn.bf16x2 %0, %1, %2;" : "=r"(d) : "r"(a), "r"(b)); return d; }
 __device__ __forceinline__ uint32_t add_bf2(uint32_t a, uint32_t b) { uint32_t d; asm("add.rn.bf16x2 %0, %1, %2;" : "=r"(d) : "r"(a), "r"(b)); return d; }
@@ -53,9 +60,12 @@ __device__ __forceinline__ uint32_t ldg32(const bf16* p) { return __ldg(reinterp
 // VARLEN: packed sequences (evo_hyena_fwd_varlen).  Grid row b is sequence b = rows [cu[b], cu[b+1]) of a (3D, T, 1) tensor map;
 // a.L is the longest length.  Every segment but a sequence's last is full (one seg_len for all), so the carry below holds unchanged;
 // a tile that reaches into the next sequence goes through the ragged-tile path (n_valid), so no foreign token enters the scan.
-template <bool STATE_ONLY, bool VARLEN = false>
+// RESUME (implies VARLEN; evo_hyena_fwd_varlen_ckpt): a sequence may start from a checkpoint table row instead of zero -- the
+// state_in / halo of the batched kernel, indexed per sequence -- and the output pass may store checkpoints as it goes.
+template <bool STATE_ONLY, bool VARLEN = false, bool RESUME = false>
 __global__ void __launch_bounds__(THREADS, 1)
-hyena_scan_ms_kernel(const __grid_constant__ CUtensorMap tmZ, const std::conditional_t<VARLEN, Args2V, Args2> a) {
+hyena_scan_ms_kernel(const __grid_constant__ CUtensorMap tmZ, const std::conditional_t<RESUME, Args2R, std::conditional_t<VARLEN, Args2V, Args2>> a) {
+  static_assert(!RESUME || VARLEN, "the resumed form is a packed-sequence form");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 127) & ~(uintptr_t)127);
   const int NST = a.nst;
@@ -144,8 +154,21 @@ hyena_scan_ms_kernel(const __grid_constant__ CUtensorMap tmZ, const std::conditi
   const uint32_t b2q = ldg32(a.fir_b + zc);
   const uint32_t dskq = ldg32(a.Dskip + ch);
 
+  long long sidx = -1;                                    // RESUME: checkpoint row this sequence starts from (clamped to the table)
+  if constexpr (RESUME) {
+    if (a.start_idx) { sidx = a.start_idx[b]; if (sidx >= a.n_table) sidx = -1; }
+  }
   if (!STATE_ONLY) {
-    if (a.state_in) {
+    if constexpr (RESUME) {
+      if (sidx >= 0) {
+#pragma unroll
+        for (int s = 0; s < NSH; ++s) {
+          const float2 v0 = __ldg(reinterpret_cast<const float2*>(a.state_table) + (sidx * a.D + ch) * NS + m0 + s);
+          const float2 v1 = __ldg(reinterpret_cast<const float2*>(a.state_table) + (sidx * a.D + ch + 1) * NS + m0 + s);
+          sr[s] = make_float2(v0.x, v1.x); si[s] = make_float2(v0.y, v1.y);
+        }
+      }
+    } else if (a.state_in) {
 #pragma unroll
       for (int s = 0; s < NSH; ++s) {
         const float2 v0 = __ldg(reinterpret_cast<const float2*>(a.state_in) + ((long long)b * a.D + ch) * NS + m0 + s);
@@ -182,6 +205,7 @@ hyena_scan_ms_kernel(const __grid_constant__ CUtensorMap tmZ, const std::conditi
     const long long t = t0 - 2 + k;
     const bf16* row = nullptr;
     if (t >= 0) row = zb + t * C3;
+    else if constexpr (RESUME) { if (sidx >= 0) row = a.halo_table + (sidx * 2 + (t + 2)) * C3; }
     else if (a.halo) row = a.halo + ((long long)b * 2 + (t + 2)) * C3;
     if (row) { ho[k] = unpack2(ldg32(row + zc + own * 128)); if (!STATE_ONLY) h2q[k] = ldg32(row + zc); }
   }
@@ -254,6 +278,10 @@ hyena_scan_ms_kernel(const __grid_constant__ CUtensorMap tmZ, const std::conditi
     }
   };
 
+  // RESUME emission: the next checkpoint row count this segment reaches (t0 is a multiple of the stage, so every checkpoint
+  // ends a full tile)
+  long long next_ck = 0;
+  if constexpr (RESUME && !STATE_ONLY) { if (a.ckpt_out) next_ck = (t0 / a.ckpt_stride + 1) * a.ckpt_stride; }
   for (int k = 0; k < n_tiles; ++k) {
     const int st = k % NST;
     mbar_wait(&full[st], (uint32_t)(k / NST) & 1);
@@ -268,6 +296,17 @@ hyena_scan_ms_kernel(const __grid_constant__ CUtensorMap tmZ, const std::conditi
     }
     __syncwarp();
     if (lane == 0) mbar_arrive(&empty[st]);
+    if constexpr (RESUME && !STATE_ONLY) {
+      if (a.ckpt_out && t0 + (long long)(k + 1) * T2 == next_ck) {     // the state after row next_ck - 1: 16 floats per thread
+        const long long row = a.ckpt_base[b] + next_ck / a.ckpt_stride - 1;
+        if (next_ck < len && row >= 0 && row < a.n_ckpt) {
+          float2* e = reinterpret_cast<float2*>(a.ckpt_out + ((row * a.D + ch) * NS) * 2) + m0;
+#pragma unroll
+          for (int s = 0; s < NSH; ++s) { e[s] = make_float2(sr[s].x, si[s].x); e[NS + s] = make_float2(sr[s].y, si[s].y); }
+        }
+        next_ck += a.ckpt_stride;
+      }
+    }
   }
 
   float* dst = nullptr;

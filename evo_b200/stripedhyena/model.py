@@ -24,7 +24,7 @@ import torch.nn.functional as F
 
 from .. import _lib
 from .._lib import (EPI_BIAS, EPI_BIAS_RESID, EPI_BIAS_ROPE, EPI_GELU_GATE, EPI_HYENA_STEP, EPI_NONE, EPI_RESID, AttnParams, AttnVarlenParams,
-                    GemmParams, GemmSmallMParams, HyenaParams, HyenaVarlenParams, check, ptr)
+                    AttnVarlenPrefixParams, GemmParams, GemmSmallMParams, HyenaParams, HyenaVarlenCkptParams, HyenaVarlenParams, check, ptr)
 from .cache import InferenceParams, RecurrentInferenceParams
 
 # kernel variants (see include/evo_b200.h); overridable for experiments
@@ -51,6 +51,22 @@ def packed_lengths(cu_seqlens, T: int):
     if len(lengths) > 65535:
         raise _lib.EvoError(f"{len(lengths)} sequences in one pack; at most 65535")
     return lengths
+
+
+class PrefixCheckpoints:
+    """What StripedHyena.prefill_checkpoints keeps of n references: logprobs (T,) fp32 of the packed references (cu: n + 1 host
+    offsets, lengths), the checkpoint stride, base (n + 1 host offsets: reference b's checkpoints are table rows
+    [base[b], base[b + 1]), row base[b] + k - 1 = the state after its first k * stride tokens), and per layer: state[i]
+    (n_ckpt, D, S, 2) fp32 and halo[i] (n_ckpt, 2, 3D) bf16 for Hyena layers, kv[i] (n, longest, 2, H, 128) bf16 for
+    attention layers."""
+
+    def __init__(self, logprobs, lengths, cu, stride, base, state, halo, kv):
+        self.logprobs, self.lengths, self.cu, self.stride, self.base = logprobs, lengths, cu, stride, base
+        self.state, self.halo, self.kv = state, halo, kv
+
+    @property
+    def n_ckpt(self) -> int:
+        return self.base[-1]
 
 
 # ----------------------------------------------------------------------------- parameter carriers
@@ -456,12 +472,37 @@ class StripedHyena(nn.Module):
             st_out = torch.empty(n, d, cfg.state_size, 2, dtype=torch.float32, device=z.device)
             fs_out = torch.empty(n, 3 * d, 2, dtype=torch.bfloat16, device=z.device)
             hp.state_out, hp.fir_state_out = st_out.data_ptr(), fs_out.data_ptr()
+        if "ckpt" in vl or "resume" in vl:
+            return self._hyena_varlen_ckpt(i, z, hp, vl)
         ws_bytes = lib.evo_hyena_fwd_varlen_workspace(C.byref(hp))
         ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=z.device)
         self._record("hyena", 8.0 * vl["T"] * d, lambda: check(lib.evo_hyena_fwd_varlen(C.byref(hp), ptr(ws), ws_bytes, self._stream()), "evo_hyena_fwd_varlen"))
         if ip is not None:
             ip.state_dict[i] = torch.view_as_complex(st_out)
             ip.fir_state_dict[i] = fs_out
+
+    def _hyena_varlen_ckpt(self, i, z, hp, vl):
+        """The checkpointed scan (evo_hyena_fwd_varlen_ckpt).  vl["ckpt"]: store this layer's (n_ckpt, D, S, 2) state table and
+        its (n_ckpt, 2, 3D) FIR history table -- z rows c - 2 and c - 1 of every checkpoint c, gathered as they are.
+        vl["resume"]: start each sequence from its start_idx row of the tables prefill_checkpoints stored for this layer."""
+        cfg, lib = self.config, _lib.lib()
+        cp = HyenaVarlenCkptParams(base=hp)
+        keep = []
+        ck = vl.get("ckpt")
+        if ck is not None and ck["n"] > 0:
+            st = torch.empty(ck["n"], cfg.hidden_size, cfg.state_size, 2, dtype=torch.float32, device=z.device)
+            cp.ckpt_states, cp.ckpt_base, cp.ckpt_stride, cp.n_ckpt = st.data_ptr(), ck["base"].data_ptr(), ck["stride"], ck["n"]
+            ck["state"][i] = st
+            ck["halo"][i] = z.index_select(0, ck["halo_rows"]).view(ck["n"], 2, 3 * cfg.hidden_size)
+        rs = vl.get("resume")
+        if rs is not None:
+            src = rs["ckpts"]
+            if src.n_ckpt > 0:
+                cp.start_idx, cp.state_table, cp.halo_table, cp.n_table = rs["start_idx"].data_ptr(), src.state[i].data_ptr(), src.halo[i].data_ptr(), src.n_ckpt
+        ws_bytes = lib.evo_hyena_fwd_varlen_ckpt_workspace(C.byref(cp))
+        ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=z.device)
+        keep.append(ws)
+        self._record("hyena", 8.0 * vl["T"] * cfg.hidden_size, lambda: check(lib.evo_hyena_fwd_varlen_ckpt(C.byref(cp), ptr(ws), ws_bytes, self._stream()), "evo_hyena_fwd_varlen_ckpt"))
 
     def _attention_block(self, i, blk, u, B, L, ip: Optional[InferenceParams], varlen=None):
         cfg = self.config
@@ -525,6 +566,20 @@ class StripedHyena(nn.Module):
         hd = d // H
         lib = _lib.lib()
         cu, n, T, mx = vl["cu"], vl["n"], vl["T"], vl["max"]
+        if "ckpt" in vl:                # the references' K,V, once per reference: the prefix every variant of it attends to
+            cache = torch.empty(n, mx, 2, H, hd, dtype=torch.bfloat16, device=qkv.device)
+            check(lib.evo_kv_append_varlen(ptr(qkv), ptr(cache), ptr(cu), n, T, mx, H, hd, mx, self._stream()), "evo_kv_append_varlen")
+            vl["ckpt"]["kv"][i] = cache
+        if "resume" in vl:
+            rs = vl["resume"]
+            cache = rs["ckpts"].kv[i]
+            ap = AttnVarlenPrefixParams(qkv=qkv.data_ptr(), out=ctx.data_ptr(), cu_seqlens=cu.data_ptr(), n_seq=n, T=T, max_seqlen=mx,
+                                        cache=cache.data_ptr(), n_cache=cache.shape[0], cache_len=cache.shape[1],
+                                        prefix_seq=rs["prefix_seq"].data_ptr(), prefix_len=rs["prefix_len"].data_ptr(),
+                                        H=H, hd=hd, softmax_scale=1.0 / math.sqrt(hd))
+            flops = 4.0 * H * hd * sum(L * (P + (L + 1) / 2.0) for L, P in zip(vl["lengths"], rs["plen"]))
+            self._record("attn", flops, lambda: check(lib.evo_attn_fwd_varlen_prefix(C.byref(ap), self._stream()), "evo_attn_fwd_varlen_prefix"))
+            return
         if ip is not None:
             if i not in ip.key_value_memory_dict:
                 ip.key_value_memory_dict[i] = torch.zeros(max(ip.max_batch_size, n), ip.max_seqlen, 2, H, hd, dtype=torch.bfloat16, device=qkv.device)
@@ -621,10 +676,11 @@ class StripedHyena(nn.Module):
         return lp, ent
 
     # ---- packed variable-length sequences: n sequences end to end as one (T,) batch, no padding ----------------------
-    def _varlen(self, ids, cu_seqlens):
+    def _varlen(self, ids, cu_seqlens, pos0=None):
         """Checks a packed call on the host before anything is launched and returns what its blocks need: the device
         cu_seqlens, n, T, the longest length, the lengths, and the (T, 64) rotary tables gathered at each row's position
-        inside its sequence (built once per forward, shared by every attention layer)."""
+        inside its sequence (built once per forward, shared by every attention layer).  pos0: n host ints, sequence b's row
+        t then sits at position pos0[b] + t (rows resumed behind a prefix)."""
         cfg = self.config
         d, H = cfg.hidden_size, cfg.num_attention_heads
         if d % H or d // H != 128 or d % 256:
@@ -639,10 +695,13 @@ class StripedHyena(nn.Module):
         lengths = packed_lengths(cu_seqlens, T)
         cu = torch.tensor([0] + lengths, dtype=torch.int64).cumsum_(0).to(dev)
         vl = {"cu": cu, "n": len(lengths), "T": T, "max": max(lengths), "lengths": lengths, "rope": None}
+        if pos0 is not None and len(pos0) != len(lengths):
+            raise _lib.EvoError(f"{len(pos0)} start positions for {len(lengths)} sequences")
         if self._attn_idxs:
             with torch.cuda.device(dev):
-                cos, sin = self._rope_tables(vl["max"], dev)
-                pos = torch.arange(T, device=dev) - torch.repeat_interleave(cu[:-1], torch.tensor(lengths, device=dev), output_size=T)
+                first = cu[:-1] if pos0 is None else cu[:-1] - torch.tensor(pos0, dtype=torch.int64).to(dev)
+                cos, sin = self._rope_tables(vl["max"] if pos0 is None else max(p + n for p, n in zip(pos0, lengths)), dev)
+                pos = torch.arange(T, device=dev) - torch.repeat_interleave(first, torch.tensor(lengths, device=dev), output_size=T)
                 vl["rope"] = (cos[pos].contiguous(), sin[pos].contiguous())
         return vl
 
@@ -671,6 +730,73 @@ class StripedHyena(nn.Module):
             targets[:-1] = x[1:]
             targets[vl["cu"][1:] - 1] = -1
             return self._score_head(u, targets, (T,), want_logprobs, want_entropy)
+
+    # ---- variant scoring: a reference's state at every stride-th row, and packed passes resumed from those states --------
+    def prefill_checkpoints(self, ids, cu_seqlens, stride):
+        """One packed forward over n references (score_tokens_packed's path) that also keeps their state every `stride` rows.
+        Checkpoint k of reference b is the model state after its first c = k * stride tokens (k >= 1, c < its length): per
+        Hyena layer the modal state and the FIR history (z rows c - 2, c - 1), stored at table row base[b] + k - 1; per
+        attention layer the reference's K,V, once, in an (n, longest, 2, H, 128) cache.  Returns a PrefixCheckpoints holding
+        them with the references' per-row logprobs (T,) fp32 (row r: the next token of its reference; 0 at each end)."""
+        if isinstance(stride, bool) or not isinstance(stride, int) or stride <= 0 or stride % 128:
+            raise _lib.EvoError(f"checkpoint stride must be a positive multiple of 128, got {stride!r}")
+        vl = self._varlen(ids, cu_seqlens)
+        dev, T = ids.device, vl["T"]
+        counts = [(n - 1) // stride for n in vl["lengths"]]
+        base = [0]
+        for c in counts:
+            base.append(base[-1] + c)
+        cu_h = [0]
+        for n in vl["lengths"]:
+            cu_h.append(cu_h[-1] + n)
+        rows = [cu_h[b] + k * stride + dr for b, c in enumerate(counts) for k in range(1, c + 1) for dr in (-2, -1)]
+        with torch.cuda.device(dev), torch.no_grad():
+            vl["ckpt"] = {"n": base[-1], "stride": stride, "base": torch.tensor(base[:-1], dtype=torch.int64, device=dev),
+                          "halo_rows": torch.tensor(rows, dtype=torch.int64, device=dev), "state": {}, "halo": {}, "kv": {}}
+            x = ids.contiguous()
+            u = self._backbone(x, 1, T, None, vl)
+            targets = torch.empty(T, dtype=torch.long, device=dev)
+            targets[:-1] = x[1:]
+            targets[vl["cu"][1:] - 1] = -1
+            lp, _ = self._score_head(u, targets, (T,), True, False)
+        ck = vl["ckpt"]
+        return PrefixCheckpoints(logprobs=lp, lengths=vl["lengths"], cu=cu_h, stride=stride, base=base, state=ck["state"],
+                                 halo=ck["halo"], kv=ck["kv"])
+
+    def score_tokens_resumed(self, ckpts, ids, cu_seqlens, start_idx, prefix_seq, prefix_len):
+        """Per-row logprobs (T,) fp32 of n packed sequences, each resumed behind a prefix of a reference of `ckpts`
+        (prefill_checkpoints): sequence b holds the tokens at positions [prefix_len[b], prefix_len[b] + len_b) of a sequence
+        whose first prefix_len[b] tokens are those of reference prefix_seq[b].  Its Hyena layers start from checkpoint row
+        start_idx[b] (-1 = from zero: prefix_len[b] must then be 0), its attention layers attend the reference's cached K,V
+        rows [0, prefix_len[b]) before its own; row t's target is the sequence's next token (0 at its last row)."""
+        n_ref = len(ckpts.lengths)
+        start_idx, prefix_seq, prefix_len = ([int(v) for v in (a.tolist() if torch.is_tensor(a) else a)] for a in (start_idx, prefix_seq, prefix_len))
+        if not len(start_idx) == len(prefix_seq) == len(prefix_len):
+            raise _lib.EvoError("start_idx, prefix_seq and prefix_len need one entry per sequence")
+        for b, (si, ps, pl) in enumerate(zip(start_idx, prefix_seq, prefix_len)):
+            if not 0 <= ps < n_ref:
+                raise _lib.EvoError(f"sequence {b}: prefix_seq {ps} outside the {n_ref} references")
+            if not 0 <= pl < ckpts.lengths[ps]:
+                raise _lib.EvoError(f"sequence {b}: prefix_len {pl} not below reference {ps}'s length {ckpts.lengths[ps]}")
+            if si == -1:
+                if pl != 0:
+                    raise _lib.EvoError(f"sequence {b}: a zero start (start_idx -1) needs prefix_len 0, got {pl}")
+            elif not ckpts.base[ps] <= si < ckpts.base[ps + 1] or (si - ckpts.base[ps] + 1) * ckpts.stride != pl:
+                raise _lib.EvoError(f"sequence {b}: start_idx {si} is not reference {ps}'s checkpoint at prefix_len {pl}")
+        vl = self._varlen(ids, cu_seqlens, pos0=prefix_len)
+        if len(start_idx) != vl["n"]:
+            raise _lib.EvoError(f"{len(start_idx)} start indices for {vl['n']} sequences")
+        dev, T = ids.device, vl["T"]
+        with torch.cuda.device(dev), torch.no_grad():
+            vl["resume"] = {"ckpts": ckpts, "start_idx": torch.tensor(start_idx, dtype=torch.int64, device=dev), "plen": prefix_len,
+                            "prefix_seq": torch.tensor(prefix_seq, dtype=torch.int64, device=dev),
+                            "prefix_len": torch.tensor(prefix_len, dtype=torch.int64, device=dev)}
+            x = ids.contiguous()
+            u = self._backbone(x, 1, T, None, vl)
+            targets = torch.empty(T, dtype=torch.long, device=dev)
+            targets[:-1] = x[1:]
+            targets[vl["cu"][1:] - 1] = -1
+            return self._score_head(u, targets, (T,), True, False)[0]
 
     # ---- decode step: small-M weight-streaming GEMM tiles + device-side position + CUDA graph ------
     def _can_step(self, ipd, B):

@@ -165,6 +165,23 @@ typedef struct {
 size_t evo_hyena_fwd_varlen_workspace(const evo_hyena_varlen_params* p);
 int evo_hyena_fwd_varlen(const evo_hyena_varlen_params* p, void* workspace, size_t workspace_bytes, void* stream);
 
+/* Checkpointed / resumed packed scan (variant scoring): evo_hyena_fwd_varlen's scan with two optional additions.
+ *   Checkpoints (ckpt_states != NULL): the state after row k*ckpt_stride - 1 of sequence b (k >= 1, k*ckpt_stride < its length)
+ *     is stored at row ckpt_base[b] + k - 1 of ckpt_states (n_ckpt, D, S, 2) fp32; ckpt_base: (n_seq) int64 DEVICE array,
+ *     ckpt_stride a positive multiple of 128.  Segment starts stay on the scan's 16-token stage (an automatic seg_len is
+ *     rounded up to a multiple of 16, a forced one must be one); a segmented call stores the states its segment carries give.
+ *   Resumed starts (start_idx != NULL): sequence b starts from modal state state_table[start_idx[b]] ((n_table, D, S, 2) fp32)
+ *     and FIR history halo_table[start_idx[b]] ((n_table, 2, 3D) bf16, the halo layout of evo_hyena_params) instead of zero;
+ *     start_idx: (n_seq) int64 DEVICE array, -1 = zero start.  fir_state_out then counts that history in front of row 0.
+ *   With neither, the results are evo_hyena_fwd_varlen's.  workspace: evo_hyena_fwd_varlen_ckpt_workspace() bytes. */
+typedef struct {
+  evo_hyena_varlen_params base;
+  float* ckpt_states; const int64_t* ckpt_base; int64_t ckpt_stride, n_ckpt;
+  const int64_t* start_idx; const float* state_table; const void* halo_table; int64_t n_table;
+} evo_hyena_varlen_ckpt_params;
+size_t evo_hyena_fwd_varlen_ckpt_workspace(const evo_hyena_varlen_ckpt_params* p);
+int evo_hyena_fwd_varlen_ckpt(const evo_hyena_varlen_ckpt_params* p, void* workspace, size_t workspace_bytes, void* stream);
+
 /* decode step: engine.step_fir + step_iir.  u (B, 3D) bf16 -> y (B, D) bf16;
  * fir_state (B, 3D, 2) bf16 and state (B, D, S, 2) fp32 are updated in place. */
 int evo_hyena_step(const void* u, void* y, void* fir_state, float* state,
@@ -227,6 +244,23 @@ typedef struct {
   float softmax_scale;
 } evo_attn_varlen_params;
 int evo_attn_fwd_varlen(const evo_attn_varlen_params* p, void* stream);
+
+/* packed causal attention behind a cached prefix (variant scoring): qkv (T, 3, H, 128) packed rows, out (T, H*128).  Sequence b's
+ * row t sits at absolute position prefix_len[b] + t and attends keys [0, prefix_len[b]) of batch row prefix_seq[b] of cache
+ * (n_cache, cache_len, 2, H, 128) bf16 -- no causal mask, rows at or past prefix_len[b] may hold anything, NaN included -- and its
+ * own rows [0, t].  prefix_seq, prefix_len: (n_seq) int64 DEVICE arrays, 0 <= prefix_len[b] <= cache_len.  Both key sources go
+ * through one online softmax with evo_attn_fwd_ws's rounding points; prefix tiles start at key 0 and own tiles at position
+ * prefix_len[b], so with prefix_len[b] % 128 == 0 the output is the bits of a batch-1 evo_attn_fwd_ws call with q_pos0 =
+ * prefix_len[b] on one cache holding the prefix and the rows, and with prefix_len[b] == 0 the bits of evo_attn_fwd_varlen. */
+typedef struct {
+  const void* qkv; void* out;
+  const int64_t* cu_seqlens; int n_seq; int64_t T, max_seqlen;
+  const void* cache; int n_cache; int64_t cache_len;
+  const int64_t* prefix_seq; const int64_t* prefix_len;
+  int H; int hd;
+  float softmax_scale;
+} evo_attn_varlen_prefix_params;
+int evo_attn_fwd_varlen_prefix(const evo_attn_varlen_prefix_params* p, void* stream);
 
 /* append k,v of qkv (B, L, 3, H, hd) at rows [pos0, pos0+L) of the KV cache
  * (max_B, max_seqlen, 2, H, hd) bf16 — MHA._update_kv_cache (mha.py:344-370). */
