@@ -4,7 +4,8 @@
 //   warpgroup 0      TMA producer  (one thread: cp.async.bulk.tensor, 128B-swizzled K-major tiles, mbarrier ring)
 //   warpgroups 1-2   consumers     (64 rows each: wgmma.mma_async m64nBNk16, fp32 accumulators in registers,
 //                                   then the fused epilogue straight from the accumulator fragments)
-// The producer runs ahead into the next tile while the consumers finish the epilogue of the current one.
+// The producer runs ahead into the next tile while the consumers finish the epilogue of the current one.  On the 256-column
+// tile the consumers stage C in shared memory and hand it to TMA stores that drain behind the next tile's MMAs.
 //
 // BN = 256: the throughput tile (variants 0 and 1).  BN = 64: the small-M weight-streaming tile (variants 2 and 3;
 // variant 3 reads W tile-major, [N/64][K/64][64][64]), N/64 CTAs keep every SM pulling weights.
@@ -30,12 +31,20 @@ constexpr int UK = 16;             // wgmma K for 16-bit inputs
 constexpr int NTHREADS = 384;
 constexpr int CONSUMER_WARPS = 8;
 
-template <int BN> struct Cfg {
+// TMA-store epilogue (256-column tile): each consumer warpgroup stages its 64 rows in two 128-column halves of its own, each
+// two 128B-swizzled 64 x 64 boxes (the swizzle caps a box row at 64 bf16): 64 KB for the two warpgroups.
+constexpr int EPI_BOX_BYTES = 64 * 64 * 2;
+constexpr int EPI_HALF_BYTES = 2 * EPI_BOX_BYTES;
+
+template <int BN, bool TMA_C = false> struct Cfg {
   static constexpr int A_BYTES = BM * BK * 2;
   static constexpr int B_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int STAGES = BN == BN_SMALL ? 8 : 4;                  // 192 KB of ring either way
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
+  // 192 KB of ring for the direct-store kernels; the TMA-store kernel gives a fourth stage to the staging (measured faster
+  // than 4 stages with one 16 KB staging half per warpgroup: DESIGN 3.2)
+  static constexpr int STAGES = BN == BN_SMALL ? 8 : (TMA_C ? 3 : 4);
+  static constexpr int STAGING_BYTES = TMA_C ? 4 * EPI_HALF_BYTES : 0;
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + STAGING_BYTES + 1024 /*align*/ + 256 /*barriers*/;
   static_assert(SMEM_BYTES <= 232448, "shared memory budget");
 };
 
@@ -117,22 +126,37 @@ __device__ __forceinline__ void lse_merge(float& m, float& s, float& w, float m2
   s = s * a + s2 * b; w = w * a + w2 * b; m = M;
 }
 
-template <int EPI, int BN>
-__global__ void __launch_bounds__(NTHREADS, 1)
-gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmArgs g) {
-  using C_ = Cfg<BN>;
+// byte offset of the bf16 pair (r, c), c even, in a staged 64 x 128 half: box c / 64, 128 B rows whose 16-byte chunks are
+// XOR-swizzled by r % 8 (the TMA SWIZZLE_128B layout).  The 8 rows a warp writes per column pair fall in 8 distinct chunks.
+__device__ __forceinline__ int stage_off(int r, int c) {
+  return (c >> 6) * EPI_BOX_BYTES + r * 128 + ((((c >> 3) & 7) ^ (r & 7)) << 4) + (c & 7) * 2;
+}
+__device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+
+// TMA_C: the C-writing epilogues of the 256-column tile go through shared memory and TMA stores (tmC), and the residual
+// arrives by TMA (tmR).  Otherwise every thread stores its fragments itself (the small-M tile, the scoring statistics and the
+// peer-scattered output, whose column -> peer mapping is not one tensor map); tmC and tmR are then unused.
+template <int EPI, int BN, bool TMA_C>
+__device__ __forceinline__ void gemm_body(const CUtensorMap* tmA, const CUtensorMap* tmB, const CUtensorMap* tmC, const CUtensorMap* tmR,
+                                          const GemmArgs& g) {
+  using C_ = Cfg<BN, TMA_C>;
   static_assert(EPI != EVO_EPI_GELU_GATE || BN == BN_BIG, "the gate epilogue needs [l1 | l2] halves of a 256-column tile");
+  static_assert(!TMA_C || (BN == BN_BIG && EPI != EPI_LSE), "TMA stores: the 256-column tile's C-writing epilogues");
+  constexpr bool RESID = EPI == EVO_EPI_BIAS_RESID || EPI == EVO_EPI_RESID;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t* smA = smem;
   uint8_t* smB = smem + C_::STAGES * C_::A_BYTES;
-  uint64_t* full = reinterpret_cast<uint64_t*>(smB + C_::STAGES * C_::B_BYTES);
+  uint8_t* staging = smB + C_::STAGES * C_::B_BYTES;
+  uint64_t* full = reinterpret_cast<uint64_t*>(staging + C_::STAGING_BYTES);
   uint64_t* empty = full + C_::STAGES;
+  uint64_t* rfull = empty + C_::STAGES;     // TMA_C with a residual: one per staging half of each consumer warpgroup
 
   const int wg = threadIdx.x >> 7, tid = threadIdx.x & 127;
   if (threadIdx.x == 0) {
-    tma_prefetch_desc(&tmA); tma_prefetch_desc(&tmB);
+    tma_prefetch_desc(tmA); tma_prefetch_desc(tmB);
     for (int i = 0; i < C_::STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], CONSUMER_WARPS); }
+    if constexpr (TMA_C && RESID) for (int i = 0; i < 4; ++i) mbar_init(&rfull[i], 1);
     fence_barrier_init();
   }
   __syncthreads();
@@ -149,9 +173,9 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         for (int kb = 0; kb < nkb; ++kb) {
           mbar_wait(&empty[stage], phase ^ 1);
           mbar_arrive_expect_tx(&full[stage], C_::STAGE_BYTES);
-          tma_load_2d(smA + stage * C_::A_BYTES, &tmA, &full[stage], kb * BK, m_blk * BM);
-          if (BN == BN_SMALL && g.b_tiled) tma_load_4d(smB + stage * C_::B_BYTES, &tmB, &full[stage], 0, 0, kb, n_blk);
-          else tma_load_2d(smB + stage * C_::B_BYTES, &tmB, &full[stage], kb * BK, n_blk * BN);
+          tma_load_2d(smA + stage * C_::A_BYTES, tmA, &full[stage], kb * BK, m_blk * BM);
+          if (BN == BN_SMALL && g.b_tiled) tma_load_4d(smB + stage * C_::B_BYTES, tmB, &full[stage], 0, 0, kb, n_blk);
+          else tma_load_2d(smB + stage * C_::B_BYTES, tmB, &full[stage], kb * BK, n_blk * BN);
           if (++stage == C_::STAGES) { stage = 0; phase ^= 1; }
         }
       }
@@ -163,8 +187,16 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     const int quad = lane & 3;
     float acc[BN / 2];
     int stage = 0; uint32_t phase = 0;
+    [[maybe_unused]] uint8_t* stg = staging + cw * 2 * EPI_HALF_BYTES;   // this warpgroup's two staging halves
+    [[maybe_unused]] uint32_t rphase = 0;                                // parity of rfull, one bit per half
+#ifdef EVO_GEMM_NO_STORE
+    constexpr bool STORE = false;     // experiment builds only: the epilogue arithmetic without residual loads or C stores
+#else
+    constexpr bool STORE = true;
+#endif
     for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
       int m_blk, n_blk; tile_coords(tile, g, m_blk, n_blk);
+      [[maybe_unused]] const int row_g = m_blk * BM + cw * 64;     // first row of this warpgroup's 64
       int prev = -1;
       for (int kb = 0; kb < nkb; ++kb) {
         mbar_wait(&full[stage], phase);
@@ -176,6 +208,23 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           else                        wgmma_m64n64k16_ss(acc, wgmma_desc_k_sw128(a0 + k * 32), wgmma_desc_k_sw128(b0 + k * 32), (kb | k) != 0);
         }
         wgmma_commit();
+        if constexpr (TMA_C) {
+          // behind the MMAs of the tile's first k-blocks: wait until the previous tile's stores have read the staging, then
+          // fetch this tile's residual into it (rows >= M arrive as zeros)
+          if (kb == (nkb > 1 ? 1 : 0) && tid == 0) {
+            tma_store_wait_read<0>();
+            if constexpr (RESID && STORE) {
+              for (int hf = 0; hf < 2; ++hf) {
+                uint64_t* bar = &rfull[cw * 2 + hf];
+                uint8_t* dst = stg + hf * EPI_HALF_BYTES;
+                const int col = n_blk * BN + hf * 128;
+                mbar_arrive_expect_tx(bar, EPI_HALF_BYTES);
+                tma_load_2d(dst, tmR, bar, col, row_g);
+                tma_load_2d(dst + EPI_BOX_BYTES, tmR, bar, col + 64, row_g);
+              }
+            }
+          }
+        }
         wgmma_wait<1>();                        // the previous k-block's MMAs are done: its stage can be refilled
         if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
         prev = stage;
@@ -187,7 +236,73 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 
       // thread (warp, lane) holds rows r0 = 16 warp + lane/4 and r0 + 8 of its 64, columns 8i + 2 (lane%4) + {0, 1}
       const long long row0 = (long long)m_blk * BM + cw * 64 + warp * 16 + (lane >> 2);
-      if constexpr (EPI == EPI_LSE) {
+      if constexpr (TMA_C) {
+        // The arithmetic and rounding points of the direct-store epilogues below, written as bf16 pairs into the staging;
+        // the TMA store clips rows >= M.  C may alias the residual: each element is read before its own store is issued.
+        constexpr bool BIAS = EPI == EVO_EPI_BIAS || EPI == EVO_EPI_BIAS_RESID;
+        constexpr int HALVES = EPI == EVO_EPI_GELU_GATE ? 1 : 2;      // the gate tile writes 128 columns
+        const int rl0 = warp * 16 + (lane >> 2);
+        if constexpr (!(RESID && STORE)) named_bar_sync(1 + cw, 128);  // after tid 0's wait for the previous stores
+#pragma unroll
+        for (int hf = 0; hf < HALVES; ++hf) {
+          uint8_t* buf = stg + hf * EPI_HALF_BYTES;
+          if constexpr (RESID && STORE) { mbar_wait(&rfull[cw * 2 + hf], (rphase >> hf) & 1); rphase ^= 1u << hf; }
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int rl = rl0 + 8 * h;
+            if constexpr (EPI == EVO_EPI_BIAS_ROPE) {
+              const bool rotate = (long long)n_blk * BN < g.rope_cols;
+              const long long l = (row0 + 8 * h) % g.rope_L;
+#pragma unroll
+              for (int j = 0; j < 8; ++j) {      // columns c and c + 64 of the head in this half
+                const int i = 16 * hf + j, c = 8 * j + 2 * quad, col = n_blk * BN + 128 * hf + c;
+                const uint32_t b1 = ld_pair(g.bias + col), b2 = ld_pair(g.bias + col + 64);
+                const float x0 = rbf(acc[4 * i + 2 * h] + bf_lo(b1)), x1 = rbf(acc[4 * i + 2 * h + 1] + bf_hi(b1));
+                const float y0 = rbf(acc[4 * (i + 8) + 2 * h] + bf_lo(b2)), y1 = rbf(acc[4 * (i + 8) + 2 * h + 1] + bf_hi(b2));
+                uint32_t o1, o2;
+                if (rotate) {
+                  const uint32_t cw2 = ld_pair(g.rope_cos + l * 64 + c), sw2 = ld_pair(g.rope_sin + l * 64 + c);
+                  const float cl = bf_lo(cw2), ch = bf_hi(cw2), sl = bf_lo(sw2), sh = bf_hi(sw2);
+                  o1 = pack_bf16(x0 * cl - y0 * sl, x1 * ch - y1 * sh);
+                  o2 = pack_bf16(x0 * sl + y0 * cl, x1 * sh + y1 * ch);
+                } else {
+                  o1 = pack_bf16(x0, x1); o2 = pack_bf16(y0, y1);
+                }
+                *reinterpret_cast<uint32_t*>(buf + stage_off(rl, c)) = o1;
+                *reinterpret_cast<uint32_t*>(buf + stage_off(rl, c + 64)) = o2;
+              }
+            } else if constexpr (EPI == EVO_EPI_GELU_GATE) {
+#pragma unroll
+              for (int i = 0; i < BN / 16; ++i) {
+                const float a0 = rbf(acc[4 * i + 2 * h]), a1 = rbf(acc[4 * i + 2 * h + 1]);
+                const float b0 = rbf(acc[4 * (i + BN / 16) + 2 * h]), b1 = rbf(acc[4 * (i + BN / 16) + 2 * h + 1]);
+                *reinterpret_cast<uint32_t*>(buf + stage_off(rl, 8 * i + 2 * quad)) = pack_bf16(rbf(gelu_erf(a0)) * b0, rbf(gelu_erf(a1)) * b1);
+              }
+            } else {
+#pragma unroll
+              for (int j = 0; j < 16; ++j) {
+                const int i = 16 * hf + j;
+                float v0 = acc[4 * i + 2 * h], v1 = acc[4 * i + 2 * h + 1];
+                if constexpr (BIAS) {
+                  const uint32_t b = ld_pair(g.bias + n_blk * BN + 8 * i + 2 * quad);
+                  v0 += bf_lo(b); v1 += bf_hi(b);
+                }
+                uint32_t* p = reinterpret_cast<uint32_t*>(buf + stage_off(rl, 8 * j + 2 * quad));
+                if constexpr (RESID) { const uint32_t r = *p; *p = pack_bf16(rbf(v0) + bf_lo(r), rbf(v1) + bf_hi(r)); }
+                else *p = pack_bf16(v0, v1);
+              }
+            }
+          }
+          fence_proxy_async_smem();           // the staging writes become visible to the TMA unit
+          named_bar_sync(1 + cw, 128);
+          if (STORE && tid == 0) {
+            const int col = EPI == EVO_EPI_GELU_GATE ? n_blk * (BN / 2) : n_blk * BN + 128 * hf;
+            tma_store_2d(tmC, buf, col, row_g);
+            tma_store_2d(tmC, buf + EPI_BOX_BYTES, col + 64, row_g);
+            tma_store_commit();
+          }
+        }
+      } else if constexpr (EPI == EPI_LSE) {
         // scoring epilogue: the 256 logits of this row's half never leave the SM.  Max / sum-exp / sum-exp-times-logit over the
         // bf16-rounded logits (the reference's logits tensor is bf16), plus the target's logit if it is in this half.
 #pragma unroll
@@ -274,7 +389,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         // bias, then the bf16 rounding of the linear output (exact in the exchanged bf16 pairs), then the residual.  The residual
         // of half a row is loaded ahead of its stores (one load latency per half row, not one per column pair); C may alias it,
         // since every element is read before the same thread writes it.
-        constexpr bool BIAS = EPI == EVO_EPI_BIAS || EPI == EVO_EPI_BIAS_RESID, RESID = EPI == EVO_EPI_BIAS_RESID || EPI == EVO_EPI_RESID;
+        constexpr bool BIAS = EPI == EVO_EPI_BIAS || EPI == EVO_EPI_BIAS_RESID;
         const int qc = quad_cols(quad);
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
@@ -321,12 +436,27 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         }
       }
     }
+    if constexpr (TMA_C) {
+      if (tid == 0) tma_store_wait_all();     // the staging must outlive the last stores' reads
+    }
   }
 }
 
 template <int EPI, int BN>
+__global__ void __launch_bounds__(NTHREADS, 1)
+gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmArgs g) {
+  gemm_body<EPI, BN, false>(&tmA, &tmB, nullptr, nullptr, g);
+}
+
+template <int EPI>
+__global__ void __launch_bounds__(NTHREADS, 1)
+gemm_wgmma_tma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmC,
+                      const __grid_constant__ CUtensorMap tmR, const GemmArgs g) {
+  gemm_body<EPI, BN_BIG, true>(&tmA, &tmB, &tmC, &tmR, g);
+}
+
+template <int EPI, int BN>
 int launch(const evo_gemm_params* p, cudaStream_t st, const long long* targets = nullptr, float4* part = nullptr) {
-  using C_ = Cfg<BN>;
   CUtensorMap tmA, tmB;
   int rc;
   if ((rc = make_tmap_2d_bf16(&tmA, p->A, (uint64_t)p->K, (uint64_t)p->M, (uint64_t)p->lda * 2, BK, BM, true))) return rc;
@@ -373,11 +503,31 @@ int launch(const evo_gemm_params* p, cudaStream_t st, const long long* targets =
     if (env_r) g.raster_n = atoi(env_r);
     if (env_g) g.group_m = std::max(1, atoi(env_g));
   }
+  const int grid = std::min(g.m_blocks * g.n_blocks, device_sm_count());
+  if constexpr (BN == BN_BIG && EPI != EPI_LSE) {
+    // C by TMA stores unless it is peer-scattered; EVO_B200_GEMM_DIRECT_STORE=1 keeps the per-thread stores (the tests'
+    // reference for the staged path)
+    const char* env_d = getenv("EVO_B200_GEMM_DIRECT_STORE");
+    if (p->n_c_peers == 0 && !(env_d && atoi(env_d))) {
+      using C_ = Cfg<BN, true>;
+      constexpr bool RESID = EPI == EVO_EPI_BIAS_RESID || EPI == EVO_EPI_RESID;
+      const uint64_t n_out = EPI == EVO_EPI_GELU_GATE ? p->N / 2 : p->N;
+      CUtensorMap tmC, tmR;
+      if ((rc = make_tmap_2d_bf16(&tmC, p->C, n_out, (uint64_t)p->M, (uint64_t)p->ldc * 2, 64, 64, true))) return rc;
+      if (RESID) { if ((rc = make_tmap_2d_bf16(&tmR, p->residual, n_out, (uint64_t)p->M, (uint64_t)p->ldr * 2, 64, 64, true))) return rc; }
+      else tmR = tmC;
+      static unsigned long long attr_done = 0;
+      auto kern = gemm_wgmma_tma_kernel<EPI>;
+      { int rc_ = ensure_dyn_smem(kern, C_::SMEM_BYTES, attr_done); if (rc_) return rc_; }
+      kern<<<grid, NTHREADS, C_::SMEM_BYTES, st>>>(tmA, tmB, tmC, tmR, g);
+      return check_launch("evo_gemm");
+    }
+  }
+  using C_ = Cfg<BN>;
   static unsigned long long attr_done = 0;     // one bit per device (the template instance has its own copy)
   auto kern = gemm_wgmma_kernel<EPI, BN>;
   { int rc_ = ensure_dyn_smem(kern, C_::SMEM_BYTES, attr_done); if (rc_) return rc_; }
-  const int n_tiles = g.m_blocks * g.n_blocks;
-  kern<<<std::min(n_tiles, device_sm_count()), NTHREADS, C_::SMEM_BYTES, st>>>(tmA, tmB, g);
+  kern<<<grid, NTHREADS, C_::SMEM_BYTES, st>>>(tmA, tmB, g);
   return check_launch("evo_gemm");
 }
 
