@@ -7,6 +7,8 @@ from .generation import generate, Generator
 from .scoring import score_sequences, positional_entropies, prepare_batch, logits_to_logprobs
 from .tokenizer import CharLevelTokenizer
 from .variants import score_variants, saturation_variants, apply_mutations
+from .embeddings import embed_sequences
 
 __all__ = ["Evo", "load_checkpoint", "generate", "Generator", "score_sequences", "positional_entropies",
-           "prepare_batch", "logits_to_logprobs", "CharLevelTokenizer", "score_variants", "saturation_variants", "apply_mutations"]
+           "prepare_batch", "logits_to_logprobs", "CharLevelTokenizer", "score_variants", "saturation_variants", "apply_mutations",
+           "embed_sequences"]

@@ -87,6 +87,16 @@ class ScoreParams(C.Structure):
                 ("M", C.c_int64), ("V", C.c_int), ("K", C.c_int64), ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t)]
 
 
+POOL_MEAN, POOL_MAX, POOL_LAST = range(3)
+
+
+class PoolVarlenParams(C.Structure):
+    _fields_ = [("x", C.c_void_p), ("ldx", C.c_int64),
+                ("cu_seqlens", C.c_void_p), ("n_seq", C.c_int), ("T", C.c_int64), ("max_seqlen", C.c_int64),
+                ("D", C.c_int), ("skip_first", C.c_int), ("mode", C.c_int),
+                ("out", C.c_void_p), ("ldo", C.c_int64)]
+
+
 class LoopParams(C.Structure):
     _fields_ = [("forced", C.c_void_p), ("n_forced", C.c_int64), ("forced_stride", C.c_int64),
                 ("picked", C.c_void_p), ("picked_stride", C.c_int64),
@@ -145,6 +155,8 @@ SIGNATURES = {
     "evo_unembed_score": (C.c_int, [C.POINTER(ScoreParams), C.c_void_p]),
     "evo_tokenize_pad": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "evo_logprobs": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p]),
+    "evo_pool_varlen_workspace": (C.c_size_t, [C.POINTER(PoolVarlenParams)]),
+    "evo_pool_varlen": (C.c_int, [C.POINTER(PoolVarlenParams), C.c_void_p, C.c_size_t, C.c_void_p]),
 }
 
 _lib = None

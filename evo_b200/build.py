@@ -12,7 +12,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libevo_b200.so")
-SOURCES = ["api.cu", "elementwise.cu", "hyena.cu", "gemm_wgmma.cu", "gemm_smallm.cu", "attention.cu", "decode.cu", "sampler.cu", "ingest.cu"]
+SOURCES = ["api.cu", "elementwise.cu", "hyena.cu", "gemm_wgmma.cu", "gemm_smallm.cu", "attention.cu", "decode.cu", "sampler.cu", "ingest.cu", "pool.cu"]
 # comparators for the GPU tests (cuBLASLt GEMM, CUDA-core attention): a separate library, never loaded by the product
 TEST_SRC = os.path.join(HERE, "..", "tests", "support", "test_support.cu")
 TEST_LIB = os.path.join(HERE, "..", "tests", "support", "libevo_b200_test.so")

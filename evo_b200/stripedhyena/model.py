@@ -15,6 +15,7 @@ from __future__ import annotations
 
 import ctypes as C
 import math
+import numbers
 import os
 from typing import Optional
 
@@ -51,6 +52,27 @@ def packed_lengths(cu_seqlens, T: int):
     if len(lengths) > 65535:
         raise _lib.EvoError(f"{len(lengths)} sequences in one pack; at most 65535")
     return lengths
+
+
+POOL_MODES = {"mean": _lib.POOL_MEAN, "max": _lib.POOL_MAX, "last": _lib.POOL_LAST}
+
+
+def resolve_layers(layers, num_layers: int):
+    """{layer: block index or "final"} of an embedding request: a layer is an int in [0, num_layers), a negative int counted
+    from the end (-1 = the last block), or "final" (the final-norm output the unembedding sees).  Raises EvoError otherwise."""
+    if isinstance(layers, (str, int)):
+        layers = [layers]
+    out = {}
+    for k in layers:
+        if isinstance(k, str) and k == "final":
+            out[k] = "final"
+        elif isinstance(k, numbers.Integral) and not isinstance(k, bool) and -num_layers <= k < num_layers:
+            out[k] = int(k) % num_layers
+        else:
+            raise _lib.EvoError(f"unknown layer {k!r}: an int in [{-num_layers}, {num_layers}) or 'final'")
+    if not out:
+        raise _lib.EvoError("no layer requested")
+    return out
 
 
 class PrefixCheckpoints:
@@ -619,25 +641,36 @@ class StripedHyena(nn.Module):
             self._gemm(u, self.unembed.weight, logits, M, V, d, EPI_NONE)
         return logits.view(B, L, V), inference_params_dict
 
-    def _backbone(self, x, B, L, inference_params_dict=None, varlen=None):
+    def _backbone(self, x, B, L, inference_params_dict=None, varlen=None, *, taps=None, last_block=None):
         """embed -> all blocks -> final norm: the (B*L, D) bf16 input of the unembedding.  varlen (from _varlen): x is a packed
-        (T,) batch run as B = 1, L = T; only the two token-mixing calls differ."""
+        (T,) batch run as B = 1, L = T; only the two token-mixing calls differ.
+        taps: {block index or "final": fn}; fn(u) is called on that block's (M, D) output (a new tensor no later block writes)
+        or on the final-norm output.  last_block: the deepest block to run.  With taps, the final norm runs only for a "final"
+        tap; the defaults run every block and the final norm, as every other caller needs."""
         M, d, V = B * L, self.config.hidden_size, self.config.vocab_size
         dev = x.device
         u = torch.empty(M, d, dtype=torch.bfloat16, device=dev)
         check(_lib.lib().evo_embed(ptr(x), int(x.dtype == torch.int64), ptr(self.embedding_layer.weight), ptr(u),
                                    M, d, V, self._stream()), "evo_embed")
         for i, blk in enumerate(self.blocks):
+            if last_block is not None and i > last_block:
+                break
             if i in self._attn_idxs:
                 ip = inference_params_dict["mha"] if inference_params_dict is not None else None
                 u = self._attention_block(i, blk, u, B, L, ip, varlen)
             else:
                 ip = inference_params_dict["hyena"] if inference_params_dict is not None else None
                 u = self._hyena_block(i, blk, u, B, L, ip, varlen)
+            if taps is not None and i in taps:
+                taps[i](u)
+        if taps is not None and "final" not in taps:
+            return u
         if self.norm is not None:
             xn = torch.empty_like(u)
             self._rmsnorm(u, self.norm.scale, xn, M)
             u = xn
+        if taps is not None:
+            taps["final"](u)
         return u
 
     def score_tokens(self, input_ids, want_logprobs=True, want_entropy=False):
@@ -730,6 +763,48 @@ class StripedHyena(nn.Module):
             targets[:-1] = x[1:]
             targets[vl["cu"][1:] - 1] = -1
             return self._score_head(u, targets, (T,), want_logprobs, want_entropy)
+
+    # ---- embeddings: block outputs of a packed forward, pooled per sequence, stopping after the deepest block asked for ----
+    def _pool(self, u, vl, skip_first, mode, out):
+        """evo_pool_varlen: out (n, D) fp32 = the pooled rows of each packed sequence of u (T, D) bf16."""
+        d, lib = self.config.hidden_size, _lib.lib()
+        pp = _lib.PoolVarlenParams(x=u.data_ptr(), ldx=u.stride(0), cu_seqlens=vl["cu"].data_ptr(), n_seq=vl["n"], T=vl["T"],
+                                   max_seqlen=vl["max"], D=d, skip_first=skip_first, mode=mode, out=out.data_ptr(), ldo=out.stride(0))
+        need = lib.evo_pool_varlen_workspace(C.byref(pp))
+        ws = torch.empty(max(need, 1), dtype=torch.uint8, device=u.device)
+        self._record("pool", 2.0 * vl["T"] * d, lambda: check(lib.evo_pool_varlen(C.byref(pp), ptr(ws), need, self._stream()), "evo_pool_varlen"))
+
+    def embed_packed(self, ids, cu_seqlens, layers=("final",), pool="mean", skip_bos=True):
+        """Sequence embeddings of n packed sequences (ids (T,), cu_seqlens as forward_packed): {layer: tensor}, keyed by the
+        layers as given (resolve_layers: block indices, negative ones counted from the end, or "final" = the final-norm output).
+        pool "mean" / "max" / "last": (n, D) fp32 per layer, over each sequence's rows without its first (the BOS) when
+        skip_bos; pool None: the (T, D) bf16 rows of the layer, every row.  Only the blocks up to the deepest layer asked for
+        run; the final norm runs only for "final", the unembedding never.  Row r holds what the full forward computes at that
+        block for that row.  Bad arguments raise EvoError before anything is launched."""
+        want = resolve_layers(layers, len(self.blocks))
+        if pool is not None and pool not in POOL_MODES:
+            raise _lib.EvoError(f"unknown pool {pool!r}: one of {sorted(POOL_MODES)} or None")
+        skip = int(bool(skip_bos)) if pool is not None else 0
+        if skip and torch.is_tensor(ids) and ids.dim() == 1 and min(packed_lengths(cu_seqlens, ids.shape[0])) <= skip:
+            raise _lib.EvoError("a sequence keeps no row to pool: every sequence needs a token after its BOS")
+        vl = self._varlen(ids, cu_seqlens)
+        d, dev, T = self.config.hidden_size, ids.device, vl["T"]
+        blocks = set(want.values())
+        got = {}
+
+        def tap(key):
+            def keep(u):
+                if pool is None:
+                    got[key] = u
+                else:
+                    got[key] = torch.empty(vl["n"], d, dtype=torch.float32, device=dev)
+                    self._pool(u, vl, skip, POOL_MODES[pool], got[key])
+            return keep
+        with torch.cuda.device(dev), torch.no_grad():
+            taps = {b: tap(b) for b in blocks}
+            self._backbone(ids.contiguous(), 1, T, None, vl, taps=taps,
+                           last_block=len(self.blocks) - 1 if "final" in blocks else max(blocks))
+        return {k: got[b] for k, b in want.items()}
 
     # ---- variant scoring: a reference's state at every stride-th row, and packed passes resumed from those states --------
     def prefill_checkpoints(self, ids, cu_seqlens, stride):

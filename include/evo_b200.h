@@ -373,6 +373,26 @@ typedef struct {
 size_t evo_unembed_score_workspace(int64_t M, int V);
 int evo_unembed_score(const evo_score_params* p, void* stream);
 
+/* ---- sequence pooling over packed rows (embeddings) ----
+ * x: T rows of D bf16 at row stride ldx (elements; x 16-byte aligned, ldx % 8 == 0); cu_seqlens: (n_seq + 1) int64 DEVICE
+ * offsets (the varlen convention above, rows clamped the same way).  Sequence b's kept rows are [cu[b] + skip_first, cu[b+1]).
+ * out[b, 0:D] (fp32, row stride ldo) =
+ *   EVO_POOL_MEAN: fp32 mean of the kept rows;  EVO_POOL_MAX: column max;  EVO_POOL_LAST: the last row, widened.
+ * A sequence with no kept row gets NaN.  The summation order of a sequence depends only on its own kept-row count, not on
+ * where it sits in the pack or on what else is packed with it, so results are deterministic and placement-independent: rows
+ * are cut into 512-row chunks counted from the first kept row, each chunk is reduced by its own CTAs, and a second pass folds
+ * the chunk partials (fp32, in the workspace) in chunk order.  No atomics.
+ * workspace: evo_pool_varlen_workspace() bytes (0 when no sequence can span more than one chunk). */
+typedef enum { EVO_POOL_MEAN = 0, EVO_POOL_MAX = 1, EVO_POOL_LAST = 2 } evo_pool_mode;
+typedef struct {
+  const void* x; int64_t ldx;
+  const int64_t* cu_seqlens; int n_seq; int64_t T, max_seqlen;
+  int D; int skip_first; int mode;
+  float* out; int64_t ldo;
+} evo_pool_varlen_params;
+size_t evo_pool_varlen_workspace(const evo_pool_varlen_params* p);
+int evo_pool_varlen(const evo_pool_varlen_params* p, void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
