@@ -26,7 +26,7 @@ import torch
 import torch.distributed as dist
 
 from . import _lib
-from ._lib import EPI_BIAS, EPI_BIAS_RESID, EPI_BIAS_ROPE, EPI_NONE, EPI_RESID, AttnParams, HyenaParams, check, ptr
+from ._lib import EPI_BIAS, EPI_BIAS_RESID, EPI_BIAS_ROPE, AttnParams, HyenaParams, check, ptr
 
 
 # attention re-shard through our own NVLink peer stores (PeerUlysses) instead of NCCL all-to-alls; "0" = NCCL Ulysses.
@@ -135,9 +135,7 @@ def _peer_attention(model, lib, pu, xn, mha, u, B, Lr, H, hd, rank, world, strea
     k = pu.calls % 2
     pu.calls += 1
     pu.epoch += 1
-    pos0 = rank * Lr
-    cos, sin = model._rope_tables(pos0 + Lr, xn.device)
-    cos_p, sin_p = cos.data_ptr() + pos0 * (hd // 2) * 2, sin.data_ptr() + pos0 * (hd // 2) * 2
+    cos_p, sin_p = model._rope_at(rank * Lr, Lr, xn.device)
     # Wqkv: bias + rotary + scatter to the head-owning ranks, tile by tile while the GEMM runs
     model._gemm(xn, mha.Wqkv.weight, None, Lr, 3 * d, d, EPI_BIAS_ROPE, bias=mha.Wqkv.bias, ldc=3 * pu.dl, rope=(cos_p, sin_p, Lr, 2 * d),
                 peers=(pu.full_ptrs[k], world, d, pu.dl, rank * Lr))
@@ -177,10 +175,8 @@ def _ulysses_attention(model, lib, qkv, ctx, B, Lr, H, hd, rank, world, group, s
     ap = AttnParams(out=out.data_ptr(), B=B, Lq=L, Lk=L, H=Hl, hd=hd, q_pos0=0, softmax_scale=1.0 / math.sqrt(hd))
     ap.q, ap.q_tok_stride, ap.q_batch_stride = full.data_ptr(), 3 * dl, L * 3 * dl
     ap.k, ap.v, ap.kv_tok_stride, ap.kv_batch_stride = full.data_ptr() + dl * 2, full.data_ptr() + 2 * dl * 2, 3 * dl, L * 3 * dl
-    n = lib.evo_attn_fwd_workspace(C.byref(ap), model.attn_variant)
-    ws = torch.empty(max(n, 1), dtype=torch.uint8, device=dev)
     causal_flops = 4.0 * B * Hl * hd * (L * (L + 1) / 2.0)
-    model._record("attn", causal_flops, lambda: check(lib.evo_attn_fwd_ws(C.byref(ap), model.attn_variant, ptr(ws), n, stream()), "evo_attn_fwd"))
+    model._launch_ws("attn", causal_flops, "evo_attn_fwd", lib.evo_attn_fwd_workspace, lib.evo_attn_fwd_ws, ap, model.attn_variant)
     # back: (B, P, Lr, Hl*hd) -> chunk p (its tokens, my heads) to rank p
     if B == 1:
         send2 = out.view(world, B, Lr, dl)            # chunk p = tokens of rank p: already contiguous
@@ -219,9 +215,8 @@ def sequence_parallel_forward(model, ids_local: torch.Tensor, rank: int, world: 
             # the transport is a collective decision: one rank on NCCL all-gathers while the others spin on peer flags would
             # hang, so every rank learns whether ALL of them have the peer path
             pu = None
-            has_bias = all(model.blocks[j].inner_mha_cls.Wqkv.bias is not None for j in model._attn_idxs)      # the rotary epilogue is bias + rotary
-            if (PEER_ULYSSES and pc is not None and B == 1 and H % world == 0 and hd == 128 and has_bias and model.attn_variant in (2, 3)
-                    and model.fused_rope and model.gemm_variant in (0, 1)):
+            rope_fused = all(model._rope_fused(model.blocks[j].inner_mha_cls) for j in model._attn_idxs)    # the peer scatter is that epilogue's
+            if PEER_ULYSSES and pc is not None and B == 1 and H % world == 0 and hd == 128 and rope_fused and model.attn_variant in (2, 3):
                 try:
                     pu = PeerUlysses(world, rank, Lr, d, H, dev, group)
                 except Exception as ex:  # noqa
@@ -246,9 +241,7 @@ def sequence_parallel_forward(model, ids_local: torch.Tensor, rank: int, world: 
     if pu is not None and pu.key != (world, rank, Lr, d, H, str(dev)):
         pu = None
     with torch.cuda.device(dev), torch.no_grad():
-        ids_local = ids_local.contiguous()
-        u = torch.empty(M, d, dtype=torch.bfloat16, device=dev)
-        check(lib.evo_embed(ptr(ids_local), int(ids_local.dtype == torch.int64), ptr(model.embedding_layer.weight), ptr(u), M, d, V, stream()), "evo_embed")
+        u = model._embed(ids_local.contiguous())
         for i, blk in enumerate(model.blocks):
             xn = torch.empty_like(u)
             model._rmsnorm(u, blk.pre_norm.scale, xn, M)
@@ -256,24 +249,15 @@ def sequence_parallel_forward(model, ids_local: torch.Tensor, rank: int, world: 
                 mha = blk.inner_mha_cls
                 ctx = _peer_attention(model, lib, pu, xn, mha, u, B, Lr, H, hd, rank, world, stream)
                 since_sync = 0           # the flag rounds are global synchronisation points
-                u2 = torch.empty_like(u)
-                model._gemm(ctx, mha.out_proj.weight, u2, M, d, d, EPI_BIAS_RESID if mha.out_proj.bias is not None else EPI_RESID, bias=mha.out_proj.bias, resid=u)
+                u2 = model._out_proj(mha, ctx, u)
             elif i in model._attn_idxs:
                 mha = blk.inner_mha_cls
                 qkv = torch.empty(M, 3 * d, dtype=torch.bfloat16, device=dev)
-                pos0 = rank * Lr
-                cos, sin = model._rope_tables(pos0 + Lr, dev)
-                cos_p, sin_p = cos.data_ptr() + pos0 * (hd // 2) * 2, sin.data_ptr() + pos0 * (hd // 2) * 2
-                if model.fused_rope and mha.Wqkv.bias is not None and hd == 128 and model.gemm_variant in (0, 1):
-                    model._gemm(xn, mha.Wqkv.weight, qkv, M, 3 * d, d, EPI_BIAS_ROPE, bias=mha.Wqkv.bias, rope=(cos_p, sin_p, Lr, 2 * d))
-                else:
-                    model._gemm(xn, mha.Wqkv.weight, qkv, M, 3 * d, d, EPI_BIAS if mha.Wqkv.bias is not None else EPI_NONE, bias=mha.Wqkv.bias)
-                    model._record("rotary", 8.0 * M * d, lambda: check(lib.evo_rotary_qk(ptr(qkv), C.c_void_p(cos_p), C.c_void_p(sin_p), B, Lr, H, hd, stream()), "evo_rotary_qk"))
+                model._qkv_rope(xn, mha, qkv, B, Lr, model._rope_at(rank * Lr, Lr, dev))
                 ctx = xn
                 _ulysses_attention(model, lib, qkv, ctx, B, Lr, H, hd, rank, world, group, stream)
                 since_sync = 0           # the all-to-all is a global synchronisation point
-                u2 = torch.empty_like(u)
-                model._gemm(ctx, mha.out_proj.weight, u2, M, d, d, EPI_BIAS_RESID if mha.out_proj.bias is not None else EPI_RESID, bias=mha.out_proj.bias, resid=u)
+                u2 = model._out_proj(mha, ctx, u)
             else:
                 f = blk.filter
                 z = torch.empty(M, 3 * d, dtype=torch.bfloat16, device=dev)
@@ -301,13 +285,10 @@ def sequence_parallel_forward(model, ids_local: torch.Tensor, rank: int, world: 
                     tails = box["t"]
                     halo = tails[rank - 1].contiguous() if rank > 0 else None
                 end = torch.empty(B, d, S, 2, dtype=torch.float32, device=dev)
-                hp = HyenaParams(z=z.data_ptr(), y=None, fir_w=f.short_filter_weight.data_ptr(), fir_b=f.short_filter_bias.data_ptr(), Dskip=f.D.data_ptr(),
-                                 poles=f.poles.data_ptr(), residues=f.residues.data_ptr(), B=B, L=Lr, D=d, S=S, nheads=H,
+                hp = HyenaParams(z=z.data_ptr(), y=None, **f.ptrs(), B=B, L=Lr, D=d, S=S, nheads=H,
                                  halo=halo.data_ptr() if halo is not None else None, state_in=None, state_out=end.data_ptr(), fir_state_out=None,
                                  force_segments=0, state_only=1)
-                n = lib.evo_hyena_fwd_workspace(C.byref(hp))
-                ws = torch.empty(max(n, 1), dtype=torch.uint8, device=dev)
-                model._record("hyena_state", 4.0 * B * Lr * d, lambda: check(lib.evo_hyena_fwd(C.byref(hp), ptr(ws), n, stream()), "evo_hyena_fwd(state)"))
+                ws, n = model._launch_ws("hyena_state", 4.0 * B * Lr * d, "evo_hyena_fwd(state)", lib.evo_hyena_fwd_workspace, lib.evo_hyena_fwd, hp)
                 if pc is not None:
                     if rank + 1 < world:   # only later shards need my end state
                         model._record("comm/peer_state", float(pc.end_bytes * (world - 1 - rank)), lambda: check(lib.evo_peer_publish(
@@ -330,10 +311,5 @@ def sequence_parallel_forward(model, ids_local: torch.Tensor, rank: int, world: 
                 u2 = torch.empty_like(u)
                 model._gemm(y, blk.out_filter_dense.weight, u2, M, d, d, EPI_BIAS_RESID, bias=blk.out_filter_dense.bias, resid=u)
             u = model._mlp_residual(i, blk, u2, M)
-        if model.norm is not None:
-            xn = torch.empty_like(u)
-            model._rmsnorm(u, model.norm.scale, xn, M)
-            u = xn
-        logits = torch.empty(M, V, dtype=torch.bfloat16, device=dev)
-        model._gemm(u, model.unembed.weight, logits, M, V, d, EPI_NONE)
+        logits = model._logits(model._final_norm(u))
     return logits.view(B, Lr, V)

@@ -17,6 +17,8 @@ import ctypes as C
 import math
 import numbers
 import os
+from dataclasses import dataclass, field
+from itertools import accumulate
 from typing import Optional
 
 import torch
@@ -89,6 +91,45 @@ class PrefixCheckpoints:
     @property
     def n_ckpt(self) -> int:
         return self.base[-1]
+
+
+@dataclass
+class _Capture:
+    """What a packed pass keeps for prefill_checkpoints (see PrefixCheckpoints), filled layer by layer into state, halo and kv;
+    base and halo_rows (the z rows c - 2, c - 1 of every checkpoint c) are on the device."""
+    n: int
+    stride: int
+    base: torch.Tensor
+    halo_rows: torch.Tensor
+    state: dict = field(default_factory=dict)
+    halo: dict = field(default_factory=dict)
+    kv: dict = field(default_factory=dict)
+
+
+@dataclass
+class _Resume:
+    """Where a packed pass resumes its sequences from (score_tokens_resumed): the three tensors are on the device, plen holds
+    prefix_len on the host."""
+    ckpts: PrefixCheckpoints
+    start_idx: torch.Tensor
+    prefix_seq: torch.Tensor
+    prefix_len: torch.Tensor
+    plen: list
+
+
+@dataclass
+class _Pack:
+    """A checked packed batch (StripedHyena._varlen): n sequences end to end as T rows, their offsets cu on the device and
+    cu_host on the host; ckpt / resume: what the pass also captures or resumes from."""
+    cu: torch.Tensor
+    cu_host: list
+    n: int
+    T: int
+    max_len: int
+    lengths: list
+    rope: Optional[tuple] = None
+    ckpt: Optional[_Capture] = None
+    resume: Optional[_Resume] = None
 
 
 # ----------------------------------------------------------------------------- parameter carriers
@@ -185,6 +226,11 @@ class _HyenaFilter(nn.Module):
         ang = (torch.rand(d, s, 1) * 2 - 1) * math.pi
         self.poles = nn.Parameter(torch.stack([mag * torch.cos(ang), mag * torch.sin(ang)], dim=-1))
         self.residues = nn.Parameter(torch.randn(d, s, 1, 2) * 0.3)
+
+    def ptrs(self):
+        """Device addresses of the five filter tensors under the field names every Hyena entry point takes, in its order."""
+        return {"fir_w": self.short_filter_weight.data_ptr(), "fir_b": self.short_filter_bias.data_ptr(), "Dskip": self.D.data_ptr(),
+                "poles": self.poles.data_ptr(), "residues": self.residues.data_ptr()}
 
 
 class _Rotary(nn.Module):
@@ -301,20 +347,17 @@ class StripedHyena(nn.Module):
 
     def load_state_dict(self, state_dict, strict: bool = True, **kw):
         out = super().load_state_dict(state_dict, strict=strict, **kw)
-        self._packed = None
-        self._decode = None
-        self._loop = None
-        self._tiled = None
+        self._invalidate()
         return out
 
     def _apply(self, fn, *a, **kw):
         out = super()._apply(fn, *a, **kw)
-        self._packed = None
-        self._rope = None
-        self._decode = None
-        self._loop = None
-        self._tiled = None
+        self._invalidate()
         return out
+
+    def _invalidate(self):
+        """Drop everything built from the parameters or buffers (rotary tables from inv_freq) and the steps that captured it."""
+        self._packed = self._rope = self._tiled = self._decode = self._loop = None
 
     # ---- weight packing (once per load / move) ---------------------------------------------
     def _ensure_packed(self):
@@ -399,8 +442,8 @@ class StripedHyena(nn.Module):
         if step is not None:
             fs, st, f = step
             p.fir_state, p.state = fs.data_ptr(), st.data_ptr()
-            p.fir_w, p.fir_b, p.Dskip = f.short_filter_weight.data_ptr(), f.short_filter_bias.data_ptr(), f.D.data_ptr()
-            p.poles, p.residues = f.poles.data_ptr(), f.residues.data_ptr()
+            for name, v in f.ptrs().items():
+                setattr(p, name, v)
         self._record(f"gemm/{N}x{K}/e{epi}/streamk", 2.0 * M * N * K, lambda: check(lib.evo_gemm_smallm(C.byref(p), self._stream()), "evo_gemm_smallm"))
 
     def _rmsnorm(self, x, scale, out, rows):
@@ -431,6 +474,29 @@ class StripedHyena(nn.Module):
         self._gemm(g, pk["w3"], out, M, d, pk["ipad"], EPI_RESID, resid=u)
         return out
 
+    def _launch_ws(self, kind, work, what, size, fn, p, *args):
+        """_record one launch of fn(&p, *args, workspace, bytes, stream) on a new workspace of size(&p, *args) bytes (at
+        least one byte is allocated, so its address is never NULL).  Returns (workspace, bytes) for a launch that reuses it."""
+        n = size(C.byref(p), *args)
+        ws = torch.empty(max(n, 1), dtype=torch.uint8, device=self.embedding_layer.weight.device)
+        self._record(kind, work, lambda: check(fn(C.byref(p), *args, ptr(ws), n, self._stream()), what))
+        return ws, n
+
+    def _hyena_state_out(self, p, n, dev):
+        """n new end states as the outputs of the scan p: (n, D, S, 2) fp32 modal states, (n, 3D, 2) bf16 FIR history."""
+        d = self.config.hidden_size
+        st = torch.empty(n, d, self.config.state_size, 2, dtype=torch.float32, device=dev)
+        fs = torch.empty(n, 3 * d, 2, dtype=torch.bfloat16, device=dev)
+        p.state_out, p.fir_state_out = st.data_ptr(), fs.data_ptr()
+        return st, fs
+
+    @staticmethod
+    def _contiguous_state(hy, i):
+        """Layer i's Hyena states in `hy`, made contiguous in place (a step reads and writes them by address): (fir, state)."""
+        st = hy.state_dict[i] = hy.state_dict[i].contiguous()
+        fs = hy.fir_state_dict[i] = hy.fir_state_dict[i].contiguous()
+        return fs, st
+
     def _hyena_block(self, i, blk, u, B, L, ip: Optional[RecurrentInferenceParams], varlen=None):
         cfg = self.config
         d, H = cfg.hidden_size, cfg.num_attention_heads
@@ -447,84 +513,93 @@ class StripedHyena(nn.Module):
         if varlen is not None:
             self._hyena_varlen(i, f, z, y, varlen, ip)
         elif have_state and L == 1:
-            st = ip.state_dict[i]
-            if not st.is_contiguous():
-                st = st.contiguous(); ip.state_dict[i] = st
-            fs = ip.fir_state_dict[i]
-            if not fs.is_contiguous():
-                fs = fs.contiguous(); ip.fir_state_dict[i] = fs
-            check(lib.evo_hyena_step(ptr(z), ptr(y), ptr(fs), ptr(torch.view_as_real(st)), ptr(f.short_filter_weight),
-                                     ptr(f.short_filter_bias), ptr(f.D), ptr(f.poles), ptr(f.residues),
+            fs, st = self._contiguous_state(ip, i)
+            check(lib.evo_hyena_step(ptr(z), ptr(y), ptr(fs), ptr(torch.view_as_real(st)), *map(C.c_void_p, f.ptrs().values()),
                                      B, d, cfg.state_size, H, self._stream()), "evo_hyena_step")
         else:
-            hp = HyenaParams(z=z.data_ptr(), y=y.data_ptr(), fir_w=f.short_filter_weight.data_ptr(), fir_b=f.short_filter_bias.data_ptr(),
-                             Dskip=f.D.data_ptr(), poles=f.poles.data_ptr(), residues=f.residues.data_ptr(),
-                             B=B, L=L, D=d, S=cfg.state_size, nheads=H, force_segments=0, state_only=0)
-            keep = []
+            hp = HyenaParams(z=z.data_ptr(), y=y.data_ptr(), **f.ptrs(), B=B, L=L, D=d, S=cfg.state_size, nheads=H, force_segments=0, state_only=0)
             if have_state:  # continued prefill: history = stored states
                 halo = ip.fir_state_dict[i].permute(0, 2, 1).contiguous()
                 sin_ = torch.view_as_real(ip.state_dict[i].contiguous()).contiguous()
                 hp.halo, hp.state_in = halo.data_ptr(), sin_.data_ptr()
-                keep += [halo, sin_]
             if ip is not None:
-                st_out = torch.empty(B, d, cfg.state_size, 2, dtype=torch.float32, device=dev)
-                fs_out = torch.empty(B, 3 * d, 2, dtype=torch.bfloat16, device=dev)
-                hp.state_out, hp.fir_state_out = st_out.data_ptr(), fs_out.data_ptr()
-            ws_bytes = lib.evo_hyena_fwd_workspace(C.byref(hp))
-            ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=dev)
-            self._record("hyena", 8.0 * B * L * d, lambda: check(lib.evo_hyena_fwd(C.byref(hp), ptr(ws), ws_bytes, self._stream()), "evo_hyena_fwd"))
+                st_out, fs_out = self._hyena_state_out(hp, B, dev)
+            self._launch_ws("hyena", 8.0 * B * L * d, "evo_hyena_fwd", lib.evo_hyena_fwd_workspace, lib.evo_hyena_fwd, hp)
             if ip is not None:
-                ip.state_dict[i] = torch.view_as_complex(st_out)
-                ip.fir_state_dict[i] = fs_out
+                ip.state_dict[i], ip.fir_state_dict[i] = torch.view_as_complex(st_out), fs_out
         u2 = torch.empty_like(u)
         self._gemm(y, blk.out_filter_dense.weight, u2, M, d, d, EPI_BIAS_RESID, bias=blk.out_filter_dense.bias, resid=u)
         return self._mlp_residual(i, blk, u2, M)
 
     def _hyena_varlen(self, i, f, z, y, vl, ip):
         """Packed sequences: one scan over all T rows (evo_hyena_fwd_varlen); with `ip`, each sequence's end states become
-        state_dict[i] (n, D, S) and fir_state_dict[i] (n, 3D, 2) as they are."""
-        cfg = self.config
-        d, n = cfg.hidden_size, vl["n"]
-        lib = _lib.lib()
-        hp = HyenaVarlenParams(z=z.data_ptr(), y=y.data_ptr(), fir_w=f.short_filter_weight.data_ptr(), fir_b=f.short_filter_bias.data_ptr(),
-                               Dskip=f.D.data_ptr(), poles=f.poles.data_ptr(), residues=f.residues.data_ptr(),
-                               cu_seqlens=vl["cu"].data_ptr(), n_seq=n, T=vl["T"], max_seqlen=vl["max"],
-                               D=d, S=cfg.state_size, nheads=cfg.num_attention_heads, seg_len=0)
-        if ip is not None:
-            st_out = torch.empty(n, d, cfg.state_size, 2, dtype=torch.float32, device=z.device)
-            fs_out = torch.empty(n, 3 * d, 2, dtype=torch.bfloat16, device=z.device)
-            hp.state_out, hp.fir_state_out = st_out.data_ptr(), fs_out.data_ptr()
-        if "ckpt" in vl or "resume" in vl:
-            return self._hyena_varlen_ckpt(i, z, hp, vl)
-        ws_bytes = lib.evo_hyena_fwd_varlen_workspace(C.byref(hp))
-        ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=z.device)
-        self._record("hyena", 8.0 * vl["T"] * d, lambda: check(lib.evo_hyena_fwd_varlen(C.byref(hp), ptr(ws), ws_bytes, self._stream()), "evo_hyena_fwd_varlen"))
-        if ip is not None:
-            ip.state_dict[i] = torch.view_as_complex(st_out)
-            ip.fir_state_dict[i] = fs_out
-
-    def _hyena_varlen_ckpt(self, i, z, hp, vl):
-        """The checkpointed scan (evo_hyena_fwd_varlen_ckpt).  vl["ckpt"]: store this layer's (n_ckpt, D, S, 2) state table and
-        its (n_ckpt, 2, 3D) FIR history table -- z rows c - 2 and c - 1 of every checkpoint c, gathered as they are.
-        vl["resume"]: start each sequence from its start_idx row of the tables prefill_checkpoints stored for this layer."""
+        state_dict[i] (n, D, S) and fir_state_dict[i] (n, 3D, 2) as they are.  With vl.ckpt or vl.resume the checkpointed scan
+        (evo_hyena_fwd_varlen_ckpt) runs instead.  vl.ckpt: store this layer's (n_ckpt, D, S, 2) state table and its
+        (n_ckpt, 2, 3D) FIR history table -- z rows c - 2 and c - 1 of every checkpoint c, gathered as they are.
+        vl.resume: start each sequence from its start_idx row of the tables prefill_checkpoints stored for this layer."""
         cfg, lib = self.config, _lib.lib()
-        cp = HyenaVarlenCkptParams(base=hp)
-        keep = []
-        ck = vl.get("ckpt")
-        if ck is not None and ck["n"] > 0:
-            st = torch.empty(ck["n"], cfg.hidden_size, cfg.state_size, 2, dtype=torch.float32, device=z.device)
-            cp.ckpt_states, cp.ckpt_base, cp.ckpt_stride, cp.n_ckpt = st.data_ptr(), ck["base"].data_ptr(), ck["stride"], ck["n"]
-            ck["state"][i] = st
-            ck["halo"][i] = z.index_select(0, ck["halo_rows"]).view(ck["n"], 2, 3 * cfg.hidden_size)
-        rs = vl.get("resume")
-        if rs is not None:
-            src = rs["ckpts"]
-            if src.n_ckpt > 0:
-                cp.start_idx, cp.state_table, cp.halo_table, cp.n_table = rs["start_idx"].data_ptr(), src.state[i].data_ptr(), src.halo[i].data_ptr(), src.n_ckpt
-        ws_bytes = lib.evo_hyena_fwd_varlen_ckpt_workspace(C.byref(cp))
-        ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=z.device)
-        keep.append(ws)
-        self._record("hyena", 8.0 * vl["T"] * cfg.hidden_size, lambda: check(lib.evo_hyena_fwd_varlen_ckpt(C.byref(cp), ptr(ws), ws_bytes, self._stream()), "evo_hyena_fwd_varlen_ckpt"))
+        d, n = cfg.hidden_size, vl.n
+        p = HyenaVarlenParams(z=z.data_ptr(), y=y.data_ptr(), **f.ptrs(), cu_seqlens=vl.cu.data_ptr(), n_seq=n, T=vl.T, max_seqlen=vl.max_len,
+                              D=d, S=cfg.state_size, nheads=cfg.num_attention_heads, seg_len=0)
+        if ip is not None:
+            st_out, fs_out = self._hyena_state_out(p, n, z.device)
+        what, size, fn = "evo_hyena_fwd_varlen", lib.evo_hyena_fwd_varlen_workspace, lib.evo_hyena_fwd_varlen
+        ck, rs = vl.ckpt, vl.resume
+        if ck is not None or rs is not None:
+            p = HyenaVarlenCkptParams(base=p)
+            what, size, fn = "evo_hyena_fwd_varlen_ckpt", lib.evo_hyena_fwd_varlen_ckpt_workspace, lib.evo_hyena_fwd_varlen_ckpt
+        if ck is not None and ck.n > 0:
+            st = torch.empty(ck.n, d, cfg.state_size, 2, dtype=torch.float32, device=z.device)
+            p.ckpt_states, p.ckpt_base, p.ckpt_stride, p.n_ckpt = st.data_ptr(), ck.base.data_ptr(), ck.stride, ck.n
+            ck.state[i] = st
+            ck.halo[i] = z.index_select(0, ck.halo_rows).view(ck.n, 2, 3 * d)
+        if rs is not None and rs.ckpts.n_ckpt > 0:
+            src = rs.ckpts
+            p.start_idx, p.state_table, p.halo_table, p.n_table = rs.start_idx.data_ptr(), src.state[i].data_ptr(), src.halo[i].data_ptr(), src.n_ckpt
+        self._launch_ws("hyena", 8.0 * vl.T * d, what, size, fn, p)
+        if ip is not None:
+            ip.state_dict[i], ip.fir_state_dict[i] = torch.view_as_complex(st_out), fs_out
+
+    def _rope_at(self, pos0, L, dev):
+        """(cos, sin) addresses of the rotary tables' rows for positions pos0 .. pos0 + L - 1."""
+        cos, sin = self._rope_tables(pos0 + L, dev)
+        off = pos0 * cos.stride(0) * cos.element_size()
+        return cos.data_ptr() + off, sin.data_ptr() + off
+
+    def _rope_fused(self, mha):
+        """Whether the Wqkv GEMM applies rotary in its epilogue (EVO_EPI_BIAS_ROPE: bias + rotary, head_dim 128, GEMM variants
+        0 and 1), where flash_attn's MHA applies it (mha.py:635-648); otherwise a second pass over qkv does."""
+        hd = self.config.hidden_size // self.config.num_attention_heads
+        return self.fused_rope and mha.Wqkv.bias is not None and hd == 128 and self.gemm_variant in (0, 1)
+
+    def _qkv_rope(self, xn, mha, qkv, B, L, rope):
+        """qkv (B*L, 3D) = Wqkv xn (+ bias), rotary on q and k from rope = (cos, sin) addresses of each sequence's L rows."""
+        cfg, lib = self.config, _lib.lib()
+        d, H = cfg.hidden_size, cfg.num_attention_heads
+        M = B * L
+        if self._rope_fused(mha):
+            self._gemm(xn, mha.Wqkv.weight, qkv, M, 3 * d, d, EPI_BIAS_ROPE, bias=mha.Wqkv.bias, rope=(*rope, L, 2 * d))
+        else:
+            self._gemm(xn, mha.Wqkv.weight, qkv, M, 3 * d, d, EPI_BIAS if mha.Wqkv.bias is not None else EPI_NONE, bias=mha.Wqkv.bias)
+            self._record("rotary", 8.0 * M * d, lambda: check(lib.evo_rotary_qk(ptr(qkv), C.c_void_p(rope[0]), C.c_void_p(rope[1]), B, L, H, d // H,
+                                                                                self._stream()), "evo_rotary_qk"))
+
+    def _out_proj(self, mha, ctx, u):
+        """u + out_proj(ctx) as a new (M, D) tensor."""
+        d = self.config.hidden_size
+        u2 = torch.empty_like(u)
+        self._gemm(ctx, mha.out_proj.weight, u2, u.shape[0], d, d, EPI_BIAS_RESID if mha.out_proj.bias is not None else EPI_RESID,
+                   bias=mha.out_proj.bias, resid=u)
+        return u2
+
+    def _kv_cache(self, ip, i, rows):
+        """Layer i's KV cache in `ip`, made on first use with `rows` rows (flash_attn/modules/mha.py:344-353; zeros instead of
+        empty: quirk Q1)."""
+        if i not in ip.key_value_memory_dict:
+            H = self.config.num_attention_heads
+            ip.key_value_memory_dict[i] = torch.zeros(rows, ip.max_seqlen, 2, H, self.config.hidden_size // H, dtype=torch.bfloat16,
+                                                      device=self.embedding_layer.weight.device)
+        return ip.key_value_memory_dict[i]
 
     def _attention_block(self, i, blk, u, B, L, ip: Optional[InferenceParams], varlen=None):
         cfg = self.config
@@ -538,47 +613,28 @@ class StripedHyena(nn.Module):
         self._rmsnorm(u, blk.pre_norm.scale, xn, M)
         qkv = torch.empty(M, 3 * d, dtype=torch.bfloat16, device=dev)
         off = int(ip.seqlen_offset) if ip is not None else 0
-        if varlen is not None:      # (T, 64) table of each row's in-sequence position: row m uses row m % rope_L, rope_L = T
-            cos_p, sin_p = (t.data_ptr() for t in varlen["rope"])
-        else:
-            cos, sin = self._rope_tables(off + L, dev)
-            hd2 = hd // 2
-            cos_p, sin_p = cos.data_ptr() + off * hd2 * 2, sin.data_ptr() + off * hd2 * 2
-        if self.fused_rope and mha.Wqkv.bias is not None and hd == 128 and self.gemm_variant in (0, 1):
-            # rotary applied in the projection's epilogue, where flash_attn's MHA applies it (mha.py:635-648): no second pass over qkv
-            self._gemm(xn, mha.Wqkv.weight, qkv, M, 3 * d, d, EPI_BIAS_ROPE, bias=mha.Wqkv.bias, rope=(cos_p, sin_p, L, 2 * d))
-        else:
-            self._gemm(xn, mha.Wqkv.weight, qkv, M, 3 * d, d, EPI_BIAS if mha.Wqkv.bias is not None else EPI_NONE, bias=mha.Wqkv.bias)
-            self._record("rotary", 8.0 * M * d, lambda: check(lib.evo_rotary_qk(ptr(qkv), C.c_void_p(cos_p), C.c_void_p(sin_p), B, L, H, hd, self._stream()), "evo_rotary_qk"))
+        # packed: the (T, 64) tables of each row's in-sequence position, read as one sequence of L = T rows
+        rope = tuple(t.data_ptr() for t in varlen.rope) if varlen is not None else self._rope_at(off, L, dev)
+        self._qkv_rope(xn, mha, qkv, B, L, rope)
         ctx = xn  # reuse
         if varlen is not None:
             self._attention_varlen(i, qkv, ctx, varlen, ip)
-            u2 = torch.empty_like(u)
-            self._gemm(ctx, mha.out_proj.weight, u2, M, d, d, EPI_BIAS_RESID if mha.out_proj.bias is not None else EPI_RESID,
-                       bias=mha.out_proj.bias, resid=u)
-            return self._mlp_residual(i, blk, u2, M)
-        ap = AttnParams(out=ctx.data_ptr(), B=B, Lq=L, H=H, hd=hd, q_pos0=off, softmax_scale=1.0 / math.sqrt(hd))
-        ap.q, ap.q_tok_stride, ap.q_batch_stride = qkv.data_ptr(), 3 * d, L * 3 * d
-        if ip is None:
-            ap.k, ap.v = qkv.data_ptr() + d * 2, qkv.data_ptr() + 2 * d * 2
-            ap.kv_tok_stride, ap.kv_batch_stride, ap.Lk = 3 * d, L * 3 * d, L
         else:
-            if i not in ip.key_value_memory_dict:  # flash_attn/modules/mha.py:344-353 (zeros instead of empty: quirk Q1)
-                ip.key_value_memory_dict[i] = torch.zeros(ip.max_batch_size, ip.max_seqlen, 2, H, hd, dtype=torch.bfloat16, device=dev)
-            cache = ip.key_value_memory_dict[i]
-            if B > cache.shape[0] or off + L > cache.shape[1]:
-                raise _lib.EvoError(f"KV cache too small: batch {B} > {cache.shape[0]} or length {off + L} > {cache.shape[1]} (mha.py:366-367)")
-            check(lib.evo_kv_append(ptr(qkv), ptr(cache), B, L, H, hd, off, cache.shape[1], self._stream()), "evo_kv_append")
-            ap.k, ap.v = cache.data_ptr(), cache.data_ptr() + d * 2
-            ap.kv_tok_stride, ap.kv_batch_stride, ap.Lk = 2 * d, cache.shape[1] * 2 * d, off + L
-        ws_bytes = lib.evo_attn_fwd_workspace(C.byref(ap), self.attn_variant)
-        ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=dev)
-        causal_flops = 4.0 * B * H * hd * (L * (off + (L + 1) / 2.0))   # QK^T + PV over the visible (query, key) pairs
-        self._record("attn", causal_flops, lambda: check(lib.evo_attn_fwd_ws(C.byref(ap), self.attn_variant, ptr(ws), ws_bytes, self._stream()), "evo_attn_fwd"))
-        u2 = torch.empty_like(u)
-        self._gemm(ctx, mha.out_proj.weight, u2, M, d, d, EPI_BIAS_RESID if mha.out_proj.bias is not None else EPI_RESID,
-                   bias=mha.out_proj.bias, resid=u)
-        return self._mlp_residual(i, blk, u2, M)
+            ap = AttnParams(out=ctx.data_ptr(), B=B, Lq=L, H=H, hd=hd, q_pos0=off, softmax_scale=1.0 / math.sqrt(hd))
+            ap.q, ap.q_tok_stride, ap.q_batch_stride = qkv.data_ptr(), 3 * d, L * 3 * d
+            if ip is None:
+                ap.k, ap.v = qkv.data_ptr() + d * 2, qkv.data_ptr() + 2 * d * 2
+                ap.kv_tok_stride, ap.kv_batch_stride, ap.Lk = 3 * d, L * 3 * d, L
+            else:
+                cache = self._kv_cache(ip, i, ip.max_batch_size)
+                if B > cache.shape[0] or off + L > cache.shape[1]:
+                    raise _lib.EvoError(f"KV cache too small: batch {B} > {cache.shape[0]} or length {off + L} > {cache.shape[1]} (mha.py:366-367)")
+                check(lib.evo_kv_append(ptr(qkv), ptr(cache), B, L, H, hd, off, cache.shape[1], self._stream()), "evo_kv_append")
+                ap.k, ap.v = cache.data_ptr(), cache.data_ptr() + d * 2
+                ap.kv_tok_stride, ap.kv_batch_stride, ap.Lk = 2 * d, cache.shape[1] * 2 * d, off + L
+            causal_flops = 4.0 * B * H * hd * (L * (off + (L + 1) / 2.0))   # QK^T + PV over the visible (query, key) pairs
+            self._launch_ws("attn", causal_flops, "evo_attn_fwd", lib.evo_attn_fwd_workspace, lib.evo_attn_fwd_ws, ap, self.attn_variant)
+        return self._mlp_residual(i, blk, self._out_proj(mha, ctx, u), M)
 
     def _attention_varlen(self, i, qkv, ctx, vl, ip):
         """Packed sequences: causal attention within each sequence (evo_attn_fwd_varlen) on the packed qkv rows; with `ip`,
@@ -587,32 +643,30 @@ class StripedHyena(nn.Module):
         d, H = cfg.hidden_size, cfg.num_attention_heads
         hd = d // H
         lib = _lib.lib()
-        cu, n, T, mx = vl["cu"], vl["n"], vl["T"], vl["max"]
-        if "ckpt" in vl:                # the references' K,V, once per reference: the prefix every variant of it attends to
+        cu, n, T, mx = vl.cu, vl.n, vl.T, vl.max_len
+        if vl.ckpt is not None:         # the references' K,V, once per reference: the prefix every variant of it attends to
             cache = torch.empty(n, mx, 2, H, hd, dtype=torch.bfloat16, device=qkv.device)
             check(lib.evo_kv_append_varlen(ptr(qkv), ptr(cache), ptr(cu), n, T, mx, H, hd, mx, self._stream()), "evo_kv_append_varlen")
-            vl["ckpt"]["kv"][i] = cache
-        if "resume" in vl:
-            rs = vl["resume"]
-            cache = rs["ckpts"].kv[i]
+            vl.ckpt.kv[i] = cache
+        if vl.resume is not None:
+            rs = vl.resume
+            cache = rs.ckpts.kv[i]
             ap = AttnVarlenPrefixParams(qkv=qkv.data_ptr(), out=ctx.data_ptr(), cu_seqlens=cu.data_ptr(), n_seq=n, T=T, max_seqlen=mx,
                                         cache=cache.data_ptr(), n_cache=cache.shape[0], cache_len=cache.shape[1],
-                                        prefix_seq=rs["prefix_seq"].data_ptr(), prefix_len=rs["prefix_len"].data_ptr(),
+                                        prefix_seq=rs.prefix_seq.data_ptr(), prefix_len=rs.prefix_len.data_ptr(),
                                         H=H, hd=hd, softmax_scale=1.0 / math.sqrt(hd))
-            flops = 4.0 * H * hd * sum(L * (P + (L + 1) / 2.0) for L, P in zip(vl["lengths"], rs["plen"]))
+            flops = 4.0 * H * hd * sum(L * (P + (L + 1) / 2.0) for L, P in zip(vl.lengths, rs.plen))
             self._record("attn", flops, lambda: check(lib.evo_attn_fwd_varlen_prefix(C.byref(ap), self._stream()), "evo_attn_fwd_varlen_prefix"))
             return
         if ip is not None:
-            if i not in ip.key_value_memory_dict:
-                ip.key_value_memory_dict[i] = torch.zeros(max(ip.max_batch_size, n), ip.max_seqlen, 2, H, hd, dtype=torch.bfloat16, device=qkv.device)
-            cache = ip.key_value_memory_dict[i]
+            cache = self._kv_cache(ip, i, max(ip.max_batch_size, n))
             if n > cache.shape[0] or mx > cache.shape[1] or not cache.is_contiguous():
                 raise _lib.EvoError(f"KV cache {tuple(cache.shape)} cannot hold {n} sequences of up to {mx} tokens")
             check(lib.evo_kv_append_varlen(ptr(qkv), ptr(cache), ptr(cu), n, T, mx, H, hd, cache.shape[1], self._stream()), "evo_kv_append_varlen")
         ap = AttnVarlenParams(q=qkv.data_ptr(), k=qkv.data_ptr() + d * 2, v=qkv.data_ptr() + 2 * d * 2, out=ctx.data_ptr(),
                               q_tok_stride=3 * d, kv_tok_stride=3 * d, cu_seqlens=cu.data_ptr(), n_seq=n, T=T, max_seqlen=mx,
                               H=H, hd=hd, softmax_scale=1.0 / math.sqrt(hd))
-        causal_flops = 4.0 * H * hd * sum(L * (L + 1) / 2.0 for L in vl["lengths"])
+        causal_flops = 4.0 * H * hd * sum(L * (L + 1) / 2.0 for L in vl.lengths)
         self._record("attn", causal_flops, lambda: check(lib.evo_attn_fwd_varlen(C.byref(ap), self._stream()), "evo_attn_fwd_varlen"))
 
     # ---- forward ---------------------------------------------------------------------------------
@@ -629,17 +683,34 @@ class StripedHyena(nn.Module):
             raise _lib.EvoError(f"input ids on {x.device}, model on {dev}")
         x = x.contiguous()
         B, L = x.shape
-        M = B * L
-        d = self.config.hidden_size
-        V = self.config.vocab_size
         if L == 1 and inference_params_dict is not None and self._can_step(inference_params_dict, B):
             with torch.cuda.device(dev), torch.no_grad():
                 return self._decode_forward(x, inference_params_dict), inference_params_dict
         with torch.cuda.device(dev), torch.no_grad():
-            u = self._backbone(x, B, L, inference_params_dict)
-            logits = torch.empty(M, V, dtype=torch.bfloat16, device=dev)
-            self._gemm(u, self.unembed.weight, logits, M, V, d, EPI_NONE)
-        return logits.view(B, L, V), inference_params_dict
+            logits = self._logits(self._backbone(x, B, L, inference_params_dict))
+        return logits.view(B, L, self.config.vocab_size), inference_params_dict
+
+    def _embed(self, x):
+        """(x.numel(), D) bf16 embedding rows of the token ids x."""
+        M, d, V = x.numel(), self.config.hidden_size, self.config.vocab_size
+        u = torch.empty(M, d, dtype=torch.bfloat16, device=x.device)
+        check(_lib.lib().evo_embed(ptr(x), int(x.dtype == torch.int64), ptr(self.embedding_layer.weight), ptr(u), M, d, V, self._stream()), "evo_embed")
+        return u
+
+    def _final_norm(self, u):
+        """The final norm of u (M, D) as a new tensor; u itself when the model has none."""
+        if self.norm is None:
+            return u
+        xn = torch.empty_like(u)
+        self._rmsnorm(u, self.norm.scale, xn, u.shape[0])
+        return xn
+
+    def _logits(self, u):
+        """(M, V) bf16 logits of the final-norm output u (M, D)."""
+        M, d, V = u.shape[0], self.config.hidden_size, self.config.vocab_size
+        logits = torch.empty(M, V, dtype=torch.bfloat16, device=u.device)
+        self._gemm(u, self.unembed.weight, logits, M, V, d, EPI_NONE)
+        return logits
 
     def _backbone(self, x, B, L, inference_params_dict=None, varlen=None, *, taps=None, last_block=None):
         """embed -> all blocks -> final norm: the (B*L, D) bf16 input of the unembedding.  varlen (from _varlen): x is a packed
@@ -647,11 +718,7 @@ class StripedHyena(nn.Module):
         taps: {block index or "final": fn}; fn(u) is called on that block's (M, D) output (a new tensor no later block writes)
         or on the final-norm output.  last_block: the deepest block to run.  With taps, the final norm runs only for a "final"
         tap; the defaults run every block and the final norm, as every other caller needs."""
-        M, d, V = B * L, self.config.hidden_size, self.config.vocab_size
-        dev = x.device
-        u = torch.empty(M, d, dtype=torch.bfloat16, device=dev)
-        check(_lib.lib().evo_embed(ptr(x), int(x.dtype == torch.int64), ptr(self.embedding_layer.weight), ptr(u),
-                                   M, d, V, self._stream()), "evo_embed")
+        u = self._embed(x)
         for i, blk in enumerate(self.blocks):
             if last_block is not None and i > last_block:
                 break
@@ -665,10 +732,7 @@ class StripedHyena(nn.Module):
                 taps[i](u)
         if taps is not None and "final" not in taps:
             return u
-        if self.norm is not None:
-            xn = torch.empty_like(u)
-            self._rmsnorm(u, self.norm.scale, xn, M)
-            u = xn
+        u = self._final_norm(u)
         if taps is not None:
             taps["final"](u)
         return u
@@ -687,8 +751,6 @@ class StripedHyena(nn.Module):
             raise _lib.EvoError(f"input ids on {input_ids.device}, model on {dev}")
         x = input_ids.contiguous()
         B, L = x.shape
-        M, d, V = B * L, self.config.hidden_size, self.config.vocab_size
-        lib = _lib.lib()
         with torch.cuda.device(dev), torch.no_grad():
             u = self._backbone(x, B, L, None)
             targets = torch.full((B, L), -1, dtype=torch.long, device=dev)
@@ -710,10 +772,9 @@ class StripedHyena(nn.Module):
 
     # ---- packed variable-length sequences: n sequences end to end as one (T,) batch, no padding ----------------------
     def _varlen(self, ids, cu_seqlens, pos0=None):
-        """Checks a packed call on the host before anything is launched and returns what its blocks need: the device
-        cu_seqlens, n, T, the longest length, the lengths, and the (T, 64) rotary tables gathered at each row's position
-        inside its sequence (built once per forward, shared by every attention layer).  pos0: n host ints, sequence b's row
-        t then sits at position pos0[b] + t (rows resumed behind a prefix)."""
+        """Checks a packed call on the host before anything is launched and returns its _Pack: what its blocks need, with
+        the (T, 64) rotary tables built once per forward and shared by every attention layer.  pos0: n host ints, sequence
+        b's row t then sits at position pos0[b] + t (rows resumed behind a prefix)."""
         cfg = self.config
         d, H = cfg.hidden_size, cfg.num_attention_heads
         if d % H or d // H != 128 or d % 256:
@@ -726,53 +787,54 @@ class StripedHyena(nn.Module):
             raise _lib.EvoError(f"input ids on {ids.device}, model on {dev}")
         T = ids.shape[0]
         lengths = packed_lengths(cu_seqlens, T)
-        cu = torch.tensor([0] + lengths, dtype=torch.int64).cumsum_(0).to(dev)
-        vl = {"cu": cu, "n": len(lengths), "T": T, "max": max(lengths), "lengths": lengths, "rope": None}
+        cu_host = list(accumulate(lengths, initial=0))
+        vl = _Pack(cu=torch.tensor(cu_host, dtype=torch.int64).to(dev), cu_host=cu_host, n=len(lengths), T=T, max_len=max(lengths), lengths=lengths)
         if pos0 is not None and len(pos0) != len(lengths):
             raise _lib.EvoError(f"{len(pos0)} start positions for {len(lengths)} sequences")
         if self._attn_idxs:
             with torch.cuda.device(dev):
-                first = cu[:-1] if pos0 is None else cu[:-1] - torch.tensor(pos0, dtype=torch.int64).to(dev)
-                cos, sin = self._rope_tables(vl["max"] if pos0 is None else max(p + n for p, n in zip(pos0, lengths)), dev)
+                first = vl.cu[:-1] if pos0 is None else vl.cu[:-1] - torch.tensor(pos0, dtype=torch.int64).to(dev)
+                cos, sin = self._rope_tables(vl.max_len if pos0 is None else max(p + n for p, n in zip(pos0, lengths)), dev)
                 pos = torch.arange(T, device=dev) - torch.repeat_interleave(first, torch.tensor(lengths, device=dev), output_size=T)
-                vl["rope"] = (cos[pos].contiguous(), sin[pos].contiguous())
+                vl.rope = (cos[pos].contiguous(), sin[pos].contiguous())
         return vl
+
+    def _packed_pass(self, ids, vl, head=None, ipd=None, *, taps=None, last_block=None):
+        """_backbone over the packed ids of vl on the model's device without autograd; returns head(u, x) of its output u and
+        the contiguous ids x, run in the same scope (u itself without a head)."""
+        with torch.cuda.device(ids.device), torch.no_grad():
+            x = ids.contiguous()
+            u = self._backbone(x, 1, vl.T, ipd, vl, taps=taps, last_block=last_block)
+            return u if head is None else head(u, x)
+
+    def _packed_score(self, u, x, vl, want_logprobs=True, want_entropy=False):
+        """_score_head over the packed rows u of ids x: row r's target is the next token of its own sequence; the last row of
+        each sequence has none (-1: logprob 0)."""
+        targets = torch.empty(vl.T, dtype=torch.long, device=x.device)
+        targets[:-1] = x[1:]
+        targets[vl.cu[1:] - 1] = -1
+        return self._score_head(u, targets, (vl.T,), want_logprobs, want_entropy)
 
     def forward_packed(self, ids, cu_seqlens):
         """Logits (T, V) bf16 of n sequences packed end to end: ids (T,), cu_seqlens n + 1 offsets (cu[0] = 0, cu[n] = T, no
         empty sequence).  Row r holds what `forward` gives at that token of its sequence alone; equal lengths give the bits of
         `forward` on the (n, L) batch.  One backbone pass over T rows: no padding, one GEMM of M = T per linear layer."""
         vl = self._varlen(ids, cu_seqlens)
-        d, V = self.config.hidden_size, self.config.vocab_size
-        dev, T = ids.device, vl["T"]
-        with torch.cuda.device(dev), torch.no_grad():
-            u = self._backbone(ids.contiguous(), 1, T, None, vl)
-            logits = torch.empty(T, V, dtype=torch.bfloat16, device=dev)
-            self._gemm(u, self.unembed.weight, logits, T, V, d, EPI_NONE)
-        return logits
+        return self._packed_pass(ids, vl, lambda u, x: self._logits(u))
 
     def score_tokens_packed(self, ids, cu_seqlens, want_logprobs=True, want_entropy=False):
         """score_tokens for packed sequences: (logprobs (T,) fp32 or None, entropy (T,) fp32 or None).  The target of row r is
         the next token of the same sequence; the last row of each sequence has none (logprob 0)."""
         vl = self._varlen(ids, cu_seqlens)
-        dev, T = ids.device, vl["T"]
-        x = ids.contiguous()
-        with torch.cuda.device(dev), torch.no_grad():
-            u = self._backbone(x, 1, T, None, vl)
-            targets = torch.empty(T, dtype=torch.long, device=dev)
-            targets[:-1] = x[1:]
-            targets[vl["cu"][1:] - 1] = -1
-            return self._score_head(u, targets, (T,), want_logprobs, want_entropy)
+        return self._packed_pass(ids, vl, lambda u, x: self._packed_score(u, x, vl, want_logprobs, want_entropy))
 
     # ---- embeddings: block outputs of a packed forward, pooled per sequence, stopping after the deepest block asked for ----
     def _pool(self, u, vl, skip_first, mode, out):
         """evo_pool_varlen: out (n, D) fp32 = the pooled rows of each packed sequence of u (T, D) bf16."""
         d, lib = self.config.hidden_size, _lib.lib()
-        pp = _lib.PoolVarlenParams(x=u.data_ptr(), ldx=u.stride(0), cu_seqlens=vl["cu"].data_ptr(), n_seq=vl["n"], T=vl["T"],
-                                   max_seqlen=vl["max"], D=d, skip_first=skip_first, mode=mode, out=out.data_ptr(), ldo=out.stride(0))
-        need = lib.evo_pool_varlen_workspace(C.byref(pp))
-        ws = torch.empty(max(need, 1), dtype=torch.uint8, device=u.device)
-        self._record("pool", 2.0 * vl["T"] * d, lambda: check(lib.evo_pool_varlen(C.byref(pp), ptr(ws), need, self._stream()), "evo_pool_varlen"))
+        pp = _lib.PoolVarlenParams(x=u.data_ptr(), ldx=u.stride(0), cu_seqlens=vl.cu.data_ptr(), n_seq=vl.n, T=vl.T,
+                                   max_seqlen=vl.max_len, D=d, skip_first=skip_first, mode=mode, out=out.data_ptr(), ldo=out.stride(0))
+        self._launch_ws("pool", 2.0 * vl.T * d, "evo_pool_varlen", lib.evo_pool_varlen_workspace, lib.evo_pool_varlen, pp)
 
     def embed_packed(self, ids, cu_seqlens, layers=("final",), pool="mean", skip_bos=True):
         """Sequence embeddings of n packed sequences (ids (T,), cu_seqlens as forward_packed): {layer: tensor}, keyed by the
@@ -788,7 +850,7 @@ class StripedHyena(nn.Module):
         if skip and torch.is_tensor(ids) and ids.dim() == 1 and min(packed_lengths(cu_seqlens, ids.shape[0])) <= skip:
             raise _lib.EvoError("a sequence keeps no row to pool: every sequence needs a token after its BOS")
         vl = self._varlen(ids, cu_seqlens)
-        d, dev, T = self.config.hidden_size, ids.device, vl["T"]
+        d, dev = self.config.hidden_size, ids.device
         blocks = set(want.values())
         got = {}
 
@@ -797,13 +859,11 @@ class StripedHyena(nn.Module):
                 if pool is None:
                     got[key] = u
                 else:
-                    got[key] = torch.empty(vl["n"], d, dtype=torch.float32, device=dev)
+                    got[key] = torch.empty(vl.n, d, dtype=torch.float32, device=dev)
                     self._pool(u, vl, skip, POOL_MODES[pool], got[key])
             return keep
-        with torch.cuda.device(dev), torch.no_grad():
-            taps = {b: tap(b) for b in blocks}
-            self._backbone(ids.contiguous(), 1, T, None, vl, taps=taps,
-                           last_block=len(self.blocks) - 1 if "final" in blocks else max(blocks))
+        self._packed_pass(ids, vl, taps={b: tap(b) for b in blocks},
+                          last_block=len(self.blocks) - 1 if "final" in blocks else max(blocks))
         return {k: got[b] for k, b in want.items()}
 
     # ---- variant scoring: a reference's state at every stride-th row, and packed passes resumed from those states --------
@@ -816,27 +876,15 @@ class StripedHyena(nn.Module):
         if isinstance(stride, bool) or not isinstance(stride, int) or stride <= 0 or stride % 128:
             raise _lib.EvoError(f"checkpoint stride must be a positive multiple of 128, got {stride!r}")
         vl = self._varlen(ids, cu_seqlens)
-        dev, T = ids.device, vl["T"]
-        counts = [(n - 1) // stride for n in vl["lengths"]]
-        base = [0]
-        for c in counts:
-            base.append(base[-1] + c)
-        cu_h = [0]
-        for n in vl["lengths"]:
-            cu_h.append(cu_h[-1] + n)
-        rows = [cu_h[b] + k * stride + dr for b, c in enumerate(counts) for k in range(1, c + 1) for dr in (-2, -1)]
-        with torch.cuda.device(dev), torch.no_grad():
-            vl["ckpt"] = {"n": base[-1], "stride": stride, "base": torch.tensor(base[:-1], dtype=torch.int64, device=dev),
-                          "halo_rows": torch.tensor(rows, dtype=torch.int64, device=dev), "state": {}, "halo": {}, "kv": {}}
-            x = ids.contiguous()
-            u = self._backbone(x, 1, T, None, vl)
-            targets = torch.empty(T, dtype=torch.long, device=dev)
-            targets[:-1] = x[1:]
-            targets[vl["cu"][1:] - 1] = -1
-            lp, _ = self._score_head(u, targets, (T,), True, False)
-        ck = vl["ckpt"]
-        return PrefixCheckpoints(logprobs=lp, lengths=vl["lengths"], cu=cu_h, stride=stride, base=base, state=ck["state"],
-                                 halo=ck["halo"], kv=ck["kv"])
+        dev = ids.device
+        counts = [(n - 1) // stride for n in vl.lengths]
+        base = list(accumulate(counts, initial=0))
+        rows = [vl.cu_host[b] + k * stride + dr for b, c in enumerate(counts) for k in range(1, c + 1) for dr in (-2, -1)]
+        ck = vl.ckpt = _Capture(n=base[-1], stride=stride, base=torch.tensor(base[:-1], dtype=torch.int64, device=dev),
+                                halo_rows=torch.tensor(rows, dtype=torch.int64, device=dev))
+        lp, _ = self._packed_pass(ids, vl, lambda u, x: self._packed_score(u, x, vl))
+        return PrefixCheckpoints(logprobs=lp, lengths=vl.lengths, cu=vl.cu_host, stride=stride, base=base, state=ck.state,
+                                 halo=ck.halo, kv=ck.kv)
 
     def score_tokens_resumed(self, ckpts, ids, cu_seqlens, start_idx, prefix_seq, prefix_len):
         """Per-row logprobs (T,) fp32 of n packed sequences, each resumed behind a prefix of a reference of `ckpts`
@@ -859,19 +907,11 @@ class StripedHyena(nn.Module):
             elif not ckpts.base[ps] <= si < ckpts.base[ps + 1] or (si - ckpts.base[ps] + 1) * ckpts.stride != pl:
                 raise _lib.EvoError(f"sequence {b}: start_idx {si} is not reference {ps}'s checkpoint at prefix_len {pl}")
         vl = self._varlen(ids, cu_seqlens, pos0=prefix_len)
-        if len(start_idx) != vl["n"]:
-            raise _lib.EvoError(f"{len(start_idx)} start indices for {vl['n']} sequences")
-        dev, T = ids.device, vl["T"]
-        with torch.cuda.device(dev), torch.no_grad():
-            vl["resume"] = {"ckpts": ckpts, "start_idx": torch.tensor(start_idx, dtype=torch.int64, device=dev), "plen": prefix_len,
-                            "prefix_seq": torch.tensor(prefix_seq, dtype=torch.int64, device=dev),
-                            "prefix_len": torch.tensor(prefix_len, dtype=torch.int64, device=dev)}
-            x = ids.contiguous()
-            u = self._backbone(x, 1, T, None, vl)
-            targets = torch.empty(T, dtype=torch.long, device=dev)
-            targets[:-1] = x[1:]
-            targets[vl["cu"][1:] - 1] = -1
-            return self._score_head(u, targets, (T,), True, False)[0]
+        if len(start_idx) != vl.n:
+            raise _lib.EvoError(f"{len(start_idx)} start indices for {vl.n} sequences")
+        on_dev = lambda v: torch.tensor(v, dtype=torch.int64, device=ids.device)
+        vl.resume = _Resume(ckpts=ckpts, start_idx=on_dev(start_idx), prefix_seq=on_dev(prefix_seq), prefix_len=on_dev(prefix_len), plen=prefix_len)
+        return self._packed_pass(ids, vl, lambda u, x: self._packed_score(u, x, vl))[0]
 
     # ---- decode step: small-M weight-streaming GEMM tiles + device-side position + CUDA graph ------
     def _can_step(self, ipd, B):
@@ -941,8 +981,7 @@ class StripedHyena(nn.Module):
             else:
                 self._gemm(a, w, out, B, N, K, epi, bias=bias, resid=resid, variant=G2)
 
-        u = torch.empty(B, d, dtype=torch.bfloat16, device=dev)
-        check(lib.evo_embed(ptr(x), int(x.dtype == torch.int64), ptr(self.embedding_layer.weight), ptr(u), B, d, V, self._stream()), "evo_embed")
+        u = self._embed(x)
         n_sm = torch.cuda.get_device_properties(dev).multi_processor_count
         nsplit = max(1, min(16, -(-8 * n_sm // (H * B))))   # >= ~4 waves of 2 CTAs/SM
         for i, blk in enumerate(self.blocks):
@@ -978,8 +1017,7 @@ class StripedHyena(nn.Module):
                     lin(xn, wsel(i, "in", blk.projections.weight), z, 3 * d, d, EPI_BIAS, bias=blk.projections.bias)
                     y = xn
                     check(lib.evo_hyena_step(ptr(z), ptr(y), ptr(hy_ip.fir_state_dict[i]), ptr(torch.view_as_real(hy_ip.state_dict[i])),
-                                             ptr(f.short_filter_weight), ptr(f.short_filter_bias), ptr(f.D), ptr(f.poles), ptr(f.residues),
-                                             B, d, cfg.state_size, H, self._stream()), "evo_hyena_step")
+                                             *map(C.c_void_p, f.ptrs().values()), B, d, cfg.state_size, H, self._stream()), "evo_hyena_step")
                 lin(y, wsel(i, "out", blk.out_filter_dense.weight), u2, d, d, EPI_BIAS_RESID, bias=blk.out_filter_dense.bias, resid=u)
             pk = self._packed[i]
             xn2 = xn
@@ -993,10 +1031,7 @@ class StripedHyena(nn.Module):
                 check(lib.evo_gelu_gate_interleaved(ptr(t), ptr(g), B, pk["ipad"], self._stream()), "evo_gelu_gate_interleaved")
             u = torch.empty_like(u2)
             lin(g, wsel(i, "w3", pk["w3"]), u, d, pk["ipad"], EPI_RESID, resid=u2)
-        if self.norm is not None:
-            xn = torch.empty_like(u)
-            self._rmsnorm(u, self.norm.scale, xn, B)
-            u = xn
+        u = self._final_norm(u)
         logits = torch.empty(B, V, dtype=torch.bfloat16, device=dev)
         lin(u, tiled["unembed"] if tiled is not None else self.unembed.weight, logits, V, d, EPI_NONE)
         return logits
@@ -1079,24 +1114,18 @@ class StripedHyena(nn.Module):
     def _prefill_packed(self, prompts, lengths, cache_len):
         cfg = self.config
         B = len(prompts)
-        d, H, V = cfg.hidden_size, cfg.num_attention_heads, cfg.vocab_size
+        d, H = cfg.hidden_size, cfg.num_attention_heads
         if lengths and max(lengths) > cache_len:
             raise _lib.EvoError(f"prompt length {max(lengths)} exceeds the KV cache ({cache_len})")
-        cu = [0]
-        for n in lengths:
-            cu.append(cu[-1] + n)
         dev = self.embedding_layer.weight.device
         ids = torch.cat([torch.as_tensor(p, dtype=torch.long) for p in prompts] or [torch.zeros(0, dtype=torch.long)]).to(dev)
-        vl = self._varlen(ids, cu)          # raises on an empty prompt, before anything is launched
-        with torch.cuda.device(dev), torch.no_grad():
-            caches = {i: torch.zeros(B, cache_len, 2, H, d // H, dtype=torch.bfloat16, device=dev) for i in sorted(self._attn_idxs)}
-            mha = InferenceParams(max_seqlen=cache_len, max_batch_size=B, seqlen_offset=0, key_value_memory_dict=caches,
-                                  lengths_per_sample=torch.tensor(lengths, dtype=torch.int64, device=dev))
-            hy = RecurrentInferenceParams(fir_filter_length=cfg.short_filter_length, state_dim=cfg.state_size, seqlen_offset=0)
-            u = self._backbone(ids, 1, vl["T"], {"mha": mha, "hyena": hy}, vl)
-            last = u.index_select(0, vl["cu"][1:] - 1)
-            head = torch.empty(B, V, dtype=torch.bfloat16, device=dev)
-            self._gemm(last, self.unembed.weight, head, B, V, d, EPI_NONE)      # the full-logits unembed's variant: the same bits per row
+        vl = self._varlen(ids, list(accumulate(lengths, initial=0)))      # raises on an empty prompt, before anything is launched
+        caches = {i: torch.zeros(B, cache_len, 2, H, d // H, dtype=torch.bfloat16, device=dev) for i in sorted(self._attn_idxs)}
+        mha = InferenceParams(max_seqlen=cache_len, max_batch_size=B, seqlen_offset=0, key_value_memory_dict=caches,
+                              lengths_per_sample=torch.tensor(lengths, dtype=torch.int64, device=dev))
+        hy = RecurrentInferenceParams(fir_filter_length=cfg.short_filter_length, state_dim=cfg.state_size, seqlen_offset=0)
+        # the last row of each prompt through the full-logits unembed: the same bits per row
+        head = self._packed_pass(ids, vl, lambda u, x: self._logits(u.index_select(0, vl.cu[1:] - 1)), {"mha": mha, "hyena": hy})
         return head, {"mha": mha, "hyena": hy}
 
     # ---- shared-prompt sampling: many rows decode from one prefill of their prompt -----------------------------------
@@ -1214,9 +1243,7 @@ class StripedHyena(nn.Module):
                 raise _lib.EvoError(f"sequence length {fill + n_steps} exceeds the KV cache ({mha_ip.key_value_memory_dict[i].shape[1]}) (mha.py:367)")
         with torch.cuda.device(dev), torch.no_grad():
             self._ensure_packed()
-            for i in list(hy_ip.state_dict):
-                hy_ip.state_dict[i] = hy_ip.state_dict[i].contiguous()
-                hy_ip.fir_state_dict[i] = hy_ip.fir_state_dict[i].contiguous()
+            key = ("loop_rows" if per_row else "loop", B) + self._step_key(ipd)
             picked = torch.empty(B, max(n_out, 1), dtype=torch.long, device=dev)
             kept = torch.empty(B, max(n_out, 1), V, dtype=torch.float32, device=dev)
             forced_c = forced.to(dev, torch.long).contiguous() if n_forced else None
@@ -1225,9 +1252,6 @@ class StripedHyena(nn.Module):
             lp = _lib.LoopParams(forced=forced_c.data_ptr() if n_forced else None, n_forced=n_forced, forced_stride=n_forced,
                                  picked=picked.data_ptr(), picked_stride=picked.shape[1], kept_logits=kept.data_ptr(), n_out=n_out,
                                  top_k=int(top_k), top_p=float(top_p), temperature=float(temperature), seed=seed, step0=0)
-            key = ("loop_rows" if per_row else "loop", B, tuple(hy_ip.state_dict[i].data_ptr() for i in sorted(hy_ip.state_dict)),
-                   tuple(hy_ip.fir_state_dict[i].data_ptr() for i in sorted(hy_ip.fir_state_dict)),
-                   tuple((mha_ip.key_value_memory_dict[i].data_ptr(), mha_ip.key_value_memory_dict[i].shape[1]) for i in sorted(mha_ip.key_value_memory_dict)))
             if shared is not None:
                 pre = mha_ip.prefix_key_value_memory_dict
                 key = ("loop_shared",) + key[1:] + (tuple((pre[i].data_ptr(), tuple(pre[i].shape)) for i in sorted(pre)),
@@ -1277,17 +1301,11 @@ class StripedHyena(nn.Module):
                 one_step()                      # eager step: allocates rope tables / workspaces the capture must not
                 done = 1
                 if self.decode_graph and n_steps > 1:
-                    g = torch.cuda.CUDAGraph()
-                    torch.cuda.synchronize()
-                    n0 = lib.evo_launch_count()
-                    with torch.cuda.graph(g):
-                        one_step()
-                    st["graph"], st["launches"], st["ptrs"] = g, lib.evo_launch_count() - n0, self._graph_ptrs()
-                    lib.evo_note_graph_replay(-st["launches"])
+                    st["graph"], st["launches"], _ = self._capture(one_step)
+                    st["ptrs"] = self._graph_ptrs()
             for _ in range(done, n_steps):
                 if st["graph"] is not None:
-                    st["graph"].replay()
-                    lib.evo_note_graph_replay(st["launches"])
+                    self._replay(st)
                 else:
                     one_step()
             if per_row:
@@ -1303,23 +1321,43 @@ class StripedHyena(nn.Module):
         """Addresses a captured step bakes in besides the state tensors: rope tables and the stream-K workspace."""
         return (tuple(t.data_ptr() for t in (self._rope or ())), self._smallm_ws.data_ptr() if self._smallm_ws is not None else 0)
 
+    def _step_key(self, ipd):
+        """The state addresses a captured step bakes in, after making every Hyena state contiguous in place: each layer's
+        modal and FIR state, and each KV cache with its length."""
+        hy_ip, kv = ipd["hyena"], ipd["mha"].key_value_memory_dict
+        for i in list(hy_ip.state_dict):
+            self._contiguous_state(hy_ip, i)
+        return (tuple(hy_ip.state_dict[i].data_ptr() for i in sorted(hy_ip.state_dict)),
+                tuple(hy_ip.fir_state_dict[i].data_ptr() for i in sorted(hy_ip.fir_state_dict)),
+                tuple((kv[i].data_ptr(), kv[i].shape[1]) for i in sorted(kv)))
+
+    @staticmethod
+    def _capture(step):
+        """Capture step() into a CUDA graph: (graph, launches per replay, what step returned).  The library counts the
+        launches made while capturing, when nothing ran: they are taken back here and counted again at each _replay."""
+        lib = _lib.lib()
+        g = torch.cuda.CUDAGraph()
+        torch.cuda.synchronize()
+        n0 = lib.evo_launch_count()
+        with torch.cuda.graph(g):
+            out = step()
+        n = lib.evo_launch_count() - n0
+        lib.evo_note_graph_replay(-n)
+        return g, n, out
+
+    @staticmethod
+    def _replay(st):
+        st["graph"].replay()
+        _lib.lib().evo_note_graph_replay(st["launches"])
+
     def _decode_forward(self, x, ipd):
         """L == 1 with populated states.  Step 1 after a prefill runs eagerly (and makes the state
         tensors contiguous / resident); step 2 captures the whole step into a CUDA graph; later
         steps replay it: one host call per token instead of ~15 launches per block."""
-        mha_ip, hy_ip = ipd["mha"], ipd["hyena"]
+        mha_ip = ipd["mha"]
         dev = x.device
         B = x.shape[0]
-        for i in list(hy_ip.state_dict):
-            if not hy_ip.state_dict[i].is_contiguous():
-                hy_ip.state_dict[i] = hy_ip.state_dict[i].contiguous()
-            if not hy_ip.fir_state_dict[i].is_contiguous():
-                hy_ip.fir_state_dict[i] = hy_ip.fir_state_dict[i].contiguous()
-        key = (B, x.dtype, tuple(hy_ip.state_dict[i].data_ptr() for i in sorted(hy_ip.state_dict)),
-               tuple(hy_ip.fir_state_dict[i].data_ptr() for i in sorted(hy_ip.fir_state_dict)),
-               tuple((mha_ip.key_value_memory_dict[i].data_ptr(), mha_ip.key_value_memory_dict[i].shape[1]) for i in sorted(mha_ip.key_value_memory_dict)),
-               # every other address the captured launches bake in: rope tables, stream-K workspace
-               tuple(t.data_ptr() for t in (self._rope or ())), self._smallm_ws.data_ptr() if self._smallm_ws is not None else 0)
+        key = (B, x.dtype) + self._step_key(ipd) + self._graph_ptrs()
         off = int(mha_ip.seqlen_offset)
         for i in mha_ip.key_value_memory_dict:
             if off >= mha_ip.key_value_memory_dict[i].shape[1]:
@@ -1334,15 +1372,7 @@ class StripedHyena(nn.Module):
             st["steps"] += 1
             return self._decode_body(st["x"], st["pos"], ipd, B).view(B, 1, -1)
         if st["graph"] is None:
-            g = torch.cuda.CUDAGraph()
-            torch.cuda.synchronize()
-            n0 = _lib.lib().evo_launch_count()
-            with torch.cuda.graph(g):
-                st["logits"] = self._decode_body(st["x"], st["pos"], ipd, B)
-            st["graph"] = g
-            st["launches"] = _lib.lib().evo_launch_count() - n0      # counted while capturing, when nothing ran: undo, then count per replay
-            _lib.lib().evo_note_graph_replay(-st["launches"])
-        st["graph"].replay()
-        _lib.lib().evo_note_graph_replay(st["launches"])
+            st["graph"], st["launches"], st["logits"] = self._capture(lambda: self._decode_body(st["x"], st["pos"], ipd, B))
+        self._replay(st)
         st["steps"] += 1
         return st["logits"].clone().view(B, 1, -1)

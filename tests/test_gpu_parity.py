@@ -633,6 +633,25 @@ def test_stateful_prefill_then_steps_equals_stateless():
         d["hyena"].seqlen_offset += 1
 
 
+def test_load_state_dict_rebuilds_rotary_tables_from_the_new_inv_freq():
+    """A checkpoint loaded after a forward carries its own fp32 rotary inv_freq: the rotary tables the earlier forward built
+    from the old buffer are dropped, so the logits are those of a model built from that checkpoint."""
+    cfg, sd, m = _tiny()
+    torch.manual_seed(2)
+    ids = (torch.randint(0, 4, (2, 200)) * 3 + 65).to(DEV)
+    before, _ = m(ids)
+    sd2 = {k: (v * 0.5 if k.endswith("rotary_emb.inv_freq") else v) for k, v in sd.items()}
+    assert sum(k.endswith("rotary_emb.inv_freq") for k in sd2) == len(cfg["attn_layer_idxs"])
+    m.load_state_dict(sd2, strict=True)
+    fresh = StripedHyena(dotdict(cfg))
+    fresh.load_state_dict(sd2, strict=True)
+    fresh = fresh.to_bfloat16_except_poles_residues().to(DEV)
+    got, _ = m(ids)
+    want, _ = fresh(ids)
+    assert not torch.equal(want, before)
+    assert torch.equal(got, want)
+
+
 def test_decode_streamk_pdl_paths_agree():
     """Decode step through (a) the 128x64 tiles without programmatic dependent launch, (b) the stream-K kernel without it,
     (c) stream-K + PDL (levels 1 and 2) inside the CUDA graph: same logits up to accumulation order, (c) repeatable bit for bit."""
