@@ -1,4 +1,4 @@
-// C-ABI plumbing: error string, launch counter, TMA descriptor encode, device query.
+// C-ABI plumbing: error string, launch counter, TMA descriptor encode, packed-geometry check, device query.
 #include "common.cuh"
 #include "../../include/evo_b200.h"
 #include <stdarg.h>
@@ -72,6 +72,12 @@ int make_tmap_nd_bf16(CUtensorMap* out, const void* base, int rank, const uint64
                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   EVO_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(rank %d) failed (%d): dims0=%llu dims1=%llu box0=%u box1=%u base=%p",
               rank, (int)r, (unsigned long long)d[0], (unsigned long long)d[1], bx[0], bx[1], base);
+  return 0;
+}
+
+int check_packed(const char* what, const int64_t* cu_seqlens, int64_t T, int64_t max_seqlen) {
+  EVO_REQUIRE(cu_seqlens != nullptr && max_seqlen > 0 && max_seqlen <= T && T < (1LL << 31),
+              "%s: needs cu_seqlens and 0 < max_seqlen <= T < 2^31 (max_seqlen %lld, T %lld)", what, (long long)max_seqlen, (long long)T);
   return 0;
 }
 

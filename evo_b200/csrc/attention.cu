@@ -276,31 +276,25 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   }
 }
 
-typedef CUresult (*encode_fn_t)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+// (HD, heads, rows, batches) map of bf16 rows of `heads` x 128 elements, tok_stride / batch_stride elements apart, read in
+// 128B-swizzled {64, 1, rows_box, 1} boxes
+int make_head_map(CUtensorMap* m, const void* base, long long heads, long long rows, long long batches, long long tok_stride,
+                  long long batch_stride, uint32_t rows_box) {
+  uint64_t dims[4] = {(uint64_t)HD, (uint64_t)heads, (uint64_t)rows, (uint64_t)batches};
+  uint64_t str[3] = {(uint64_t)HD * 2, (uint64_t)tok_stride * 2, (uint64_t)batch_stride * 2};
+  uint32_t box[4] = {64, 1, rows_box, 1};
+  return make_tmap_nd_bf16(m, base, 4, dims, str, box, true);
+}
 
-int make_tmap_4d(CUtensorMap* out, const void* base, const uint64_t dims[4], const uint64_t strides_bytes[3], const uint32_t box[4]) {
-  static encode_fn_t fn = nullptr;
-  if (!fn) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult qr;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qr) != cudaSuccess || !p) {
-      set_error("cuTensorMapEncodeTiled entry point not available");
-      return -1;
-    }
-    fn = (encode_fn_t)p;
-  }
-  cuuint64_t d[4] = {dims[0], dims[1], dims[2], dims[3]};
-  cuuint64_t s[3] = {strides_bytes[0], strides_bytes[1], strides_bytes[2]};
-  cuuint32_t bx[4] = {box[0], box[1], box[2], box[3]};
-  cuuint32_t es[4] = {1, 1, 1, 1};
-  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(base), d, s, bx, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                  CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  EVO_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(4d) failed (%d): dims=%llu,%llu,%llu,%llu strides=%llu,%llu,%llu",
-              (int)r, (unsigned long long)d[0], (unsigned long long)d[1], (unsigned long long)d[2], (unsigned long long)d[3],
-              (unsigned long long)s[0], (unsigned long long)s[1], (unsigned long long)s[2]);
-  return 0;
+// one CTA per (128 query rows, head, sequence); A is the argument struct of the <VARLEN, PREFIX> form
+template <bool VARLEN, bool PREFIX, typename A>
+int launch_attn(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV, const A& a, cudaStream_t st, const char* what) {
+  static unsigned long long done = 0;      // one mask per kernel: the limit is an attribute of each kernel
+  int rc;
+  if ((rc = ensure_dyn_smem(attn_fwd_kernel<VARLEN, PREFIX>, ATT_SMEM, done))) return rc;
+  dim3 grid((unsigned)((a.Lq + BQ - 1) / BQ), a.H, a.B);
+  attn_fwd_kernel<VARLEN, PREFIX><<<grid, ATT_THREADS, ATT_SMEM, st>>>(tmQ, tmK, tmV, a);
+  return check_launch(what);
 }
 
 }  // namespace
@@ -327,97 +321,52 @@ extern "C" int evo_attn_fwd_ws(const evo_attn_params* p, int variant, void* work
                 "evo_attn_fwd: peer-scattered output needs B == 1, 1..8 peers covering Lq rows, 16-byte aligned strides");
   }
   if (p->Lq == 0 || p->B == 0) return 0;
-  cudaStream_t st = (cudaStream_t)stream;
   CUtensorMap tmQ, tmK, tmV;
   int rc;
-  {
-    uint64_t dims[4] = {(uint64_t)HD, (uint64_t)p->H, (uint64_t)p->Lq, (uint64_t)p->B};
-    uint64_t str[3] = {(uint64_t)HD * 2, (uint64_t)p->q_tok_stride * 2, (uint64_t)p->q_batch_stride * 2};
-    uint32_t box[4] = {64, 1, BQ, 1};
-    if ((rc = make_tmap_4d(&tmQ, p->q, dims, str, box))) return rc;
-  }
-  {
-    uint64_t dims[4] = {(uint64_t)HD, (uint64_t)p->H, (uint64_t)p->Lk, (uint64_t)p->B};
-    uint64_t str[3] = {(uint64_t)HD * 2, (uint64_t)p->kv_tok_stride * 2, (uint64_t)p->kv_batch_stride * 2};
-    uint32_t box[4] = {64, 1, BKV, 1};
-    if ((rc = make_tmap_4d(&tmK, p->k, dims, str, box))) return rc;
-    if ((rc = make_tmap_4d(&tmV, p->v, dims, str, box))) return rc;
-  }
+  if ((rc = make_head_map(&tmQ, p->q, p->H, p->Lq, p->B, p->q_tok_stride, p->q_batch_stride, BQ))) return rc;
+  if ((rc = make_head_map(&tmK, p->k, p->H, p->Lk, p->B, p->kv_tok_stride, p->kv_batch_stride, BKV))) return rc;
+  if ((rc = make_head_map(&tmV, p->v, p->H, p->Lk, p->B, p->kv_tok_stride, p->kv_batch_stride, BKV))) return rc;
   AttArgs a;
   a.out = (bf16*)p->out; a.B = p->B; a.H = p->H; a.Lq = p->Lq; a.Lk = p->Lk; a.q_pos0 = p->q_pos0;
   a.scale_log2 = p->softmax_scale * 1.4426950408889634f;
   a.n_out_peers = p->n_out_peers; a.out_rows_per_peer = p->out_rows_per_peer; a.out_row_stride = p->out_row_stride; a.out_col0 = p->out_col0;
   for (int i = 0; i < 8; ++i) a.out_peer[i] = i < p->n_out_peers ? (bf16*)p->out_peers[i] : nullptr;
-  dim3 grid((unsigned)((p->Lq + BQ - 1) / BQ), p->H, p->B);
-  static unsigned long long done = 0;
-  if ((rc = ensure_dyn_smem(attn_fwd_kernel<false>, ATT_SMEM, done))) return rc;
-  attn_fwd_kernel<false><<<grid, ATT_THREADS, ATT_SMEM, st>>>(tmQ, tmK, tmV, a);
-  return check_launch("evo_attn_fwd");
+  return launch_attn<false, false>(tmQ, tmK, tmV, a, (cudaStream_t)stream, "evo_attn_fwd");
 }
 
 extern "C" int evo_attn_fwd_varlen(const evo_attn_varlen_params* p, void* stream) {
   EVO_REQUIRE(p->hd == HD, "evo_attn_fwd_varlen: head_dim %d unsupported (kernel is specialised for 128)", p->hd);
   EVO_REQUIRE(p->q_tok_stride % 8 == 0 && p->kv_tok_stride % 8 == 0, "evo_attn_fwd_varlen: strides must be multiples of 8 elements");
   EVO_REQUIRE(p->n_seq > 0 && p->n_seq <= 65535 && p->H > 0 && p->H <= 65535, "evo_attn_fwd_varlen: bad sequence count %d or head count %d", p->n_seq, p->H);
-  EVO_REQUIRE(p->cu_seqlens != nullptr && p->max_seqlen > 0 && p->max_seqlen <= p->T && p->T < (1LL << 31),
-              "evo_attn_fwd_varlen: needs cu_seqlens and 0 < max_seqlen <= T < 2^31 (max_seqlen %lld, T %lld)", (long long)p->max_seqlen, (long long)p->T);
-  cudaStream_t st = (cudaStream_t)stream;
-  CUtensorMap tmQ, tmK, tmV;
   int rc;
-  {
-    uint64_t dims[4] = {(uint64_t)HD, (uint64_t)p->H, (uint64_t)p->T, 1};
-    uint64_t str[3] = {(uint64_t)HD * 2, (uint64_t)p->q_tok_stride * 2, (uint64_t)p->T * p->q_tok_stride * 2};
-    uint32_t box[4] = {64, 1, BQ, 1};
-    if ((rc = make_tmap_4d(&tmQ, p->q, dims, str, box))) return rc;
-  }
-  {
-    uint64_t dims[4] = {(uint64_t)HD, (uint64_t)p->H, (uint64_t)p->T, 1};
-    uint64_t str[3] = {(uint64_t)HD * 2, (uint64_t)p->kv_tok_stride * 2, (uint64_t)p->T * p->kv_tok_stride * 2};
-    uint32_t box[4] = {64, 1, BKV, 1};
-    if ((rc = make_tmap_4d(&tmK, p->k, dims, str, box))) return rc;
-    if ((rc = make_tmap_4d(&tmV, p->v, dims, str, box))) return rc;
-  }
+  if ((rc = check_packed("evo_attn_fwd_varlen", p->cu_seqlens, p->T, p->max_seqlen))) return rc;
+  CUtensorMap tmQ, tmK, tmV;
+  if ((rc = make_head_map(&tmQ, p->q, p->H, p->T, 1, p->q_tok_stride, p->T * p->q_tok_stride, BQ))) return rc;
+  if ((rc = make_head_map(&tmK, p->k, p->H, p->T, 1, p->kv_tok_stride, p->T * p->kv_tok_stride, BKV))) return rc;
+  if ((rc = make_head_map(&tmV, p->v, p->H, p->T, 1, p->kv_tok_stride, p->T * p->kv_tok_stride, BKV))) return rc;
   AttArgsV a = {};
   a.out = (bf16*)p->out; a.B = p->n_seq; a.H = p->H; a.Lq = a.Lk = p->max_seqlen; a.q_pos0 = 0;
   a.scale_log2 = p->softmax_scale * 1.4426950408889634f;
   a.cu_seqlens = (const long long*)p->cu_seqlens; a.T = p->T;
-  dim3 grid((unsigned)((p->max_seqlen + BQ - 1) / BQ), p->H, p->n_seq);
-  static unsigned long long done = 0;
-  if ((rc = ensure_dyn_smem(attn_fwd_kernel<true>, ATT_SMEM, done))) return rc;
-  attn_fwd_kernel<true><<<grid, ATT_THREADS, ATT_SMEM, st>>>(tmQ, tmK, tmV, a);
-  return check_launch("evo_attn_fwd_varlen");
+  return launch_attn<true, false>(tmQ, tmK, tmV, a, (cudaStream_t)stream, "evo_attn_fwd_varlen");
 }
 
 extern "C" int evo_attn_fwd_varlen_prefix(const evo_attn_varlen_prefix_params* p, void* stream) {
   EVO_REQUIRE(p->hd == HD, "evo_attn_fwd_varlen_prefix: head_dim %d unsupported (kernel is specialised for 128)", p->hd);
   EVO_REQUIRE(p->n_seq > 0 && p->n_seq <= 65535 && p->H > 0 && 3 * p->H <= 65535, "evo_attn_fwd_varlen_prefix: bad sequence count %d or head count %d", p->n_seq, p->H);
-  EVO_REQUIRE(p->cu_seqlens != nullptr && p->max_seqlen > 0 && p->max_seqlen <= p->T && p->T < (1LL << 31),
-              "evo_attn_fwd_varlen_prefix: needs cu_seqlens and 0 < max_seqlen <= T < 2^31 (max_seqlen %lld, T %lld)", (long long)p->max_seqlen, (long long)p->T);
+  int rc;
+  if ((rc = check_packed("evo_attn_fwd_varlen_prefix", p->cu_seqlens, p->T, p->max_seqlen))) return rc;
   EVO_REQUIRE(p->cache != nullptr && p->n_cache > 0 && p->cache_len > 0 && p->cache_len < (1LL << 31) && p->prefix_seq != nullptr && p->prefix_len != nullptr,
               "evo_attn_fwd_varlen_prefix: needs a cache of n_cache > 0 rows of 0 < cache_len < 2^31 keys, prefix_seq and prefix_len");
-  cudaStream_t st = (cudaStream_t)stream;
+  // q, k, v of the packed rows are heads h, H + h, 2H + h of one map; k, v of the cache are heads h, H + h of the other
   CUtensorMap tmQKV, tmC;
-  int rc;
-  {
-    uint64_t dims[4] = {(uint64_t)HD, (uint64_t)3 * p->H, (uint64_t)p->T, 1};
-    uint64_t str[3] = {(uint64_t)HD * 2, (uint64_t)3 * p->H * HD * 2, (uint64_t)p->T * 3 * p->H * HD * 2};
-    uint32_t box[4] = {64, 1, BQ, 1};
-    if ((rc = make_tmap_4d(&tmQKV, p->qkv, dims, str, box))) return rc;
-  }
-  {
-    uint64_t dims[4] = {(uint64_t)HD, (uint64_t)2 * p->H, (uint64_t)p->cache_len, (uint64_t)p->n_cache};
-    uint64_t str[3] = {(uint64_t)HD * 2, (uint64_t)2 * p->H * HD * 2, (uint64_t)p->cache_len * 2 * p->H * HD * 2};
-    uint32_t box[4] = {64, 1, BKV, 1};
-    if ((rc = make_tmap_4d(&tmC, p->cache, dims, str, box))) return rc;
-  }
+  const long long row = 3LL * p->H * HD, cache_row = 2LL * p->H * HD;
+  if ((rc = make_head_map(&tmQKV, p->qkv, 3LL * p->H, p->T, 1, row, p->T * row, BQ))) return rc;
+  if ((rc = make_head_map(&tmC, p->cache, 2LL * p->H, p->cache_len, p->n_cache, cache_row, p->cache_len * cache_row, BKV))) return rc;
   AttArgsP a = {};
   a.out = (bf16*)p->out; a.B = p->n_seq; a.H = p->H; a.Lq = a.Lk = p->max_seqlen; a.q_pos0 = 0;
   a.scale_log2 = p->softmax_scale * 1.4426950408889634f;
   a.cu_seqlens = (const long long*)p->cu_seqlens; a.T = p->T;
   a.prefix_seq = (const long long*)p->prefix_seq; a.prefix_len = (const long long*)p->prefix_len; a.cache_len = p->cache_len; a.n_cache = p->n_cache;
-  dim3 grid((unsigned)((p->max_seqlen + BQ - 1) / BQ), p->H, p->n_seq);
-  static unsigned long long done = 0;
-  if ((rc = ensure_dyn_smem(attn_fwd_kernel<true, true>, ATT_SMEM, done))) return rc;
-  attn_fwd_kernel<true, true><<<grid, ATT_THREADS, ATT_SMEM, st>>>(tmQKV, tmC, tmC, a);
-  return check_launch("evo_attn_fwd_varlen_prefix");
+  return launch_attn<true, true>(tmQKV, tmC, tmC, a, (cudaStream_t)stream, "evo_attn_fwd_varlen_prefix");
 }

@@ -146,6 +146,10 @@ int make_tmap_2d_bf16(CUtensorMap* out, const void* base, uint64_t inner, uint64
 int make_tmap_nd_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
                       const uint32_t* box, bool swizzle128);
 
+// host: the packed-sequence geometry every varlen entry point needs (cu_seqlens given, 0 < max_seqlen <= T < 2^31); on failure
+// returns -1 with the reason under `what`, the entry point's name.  Touches no device state.
+int check_packed(const char* what, const int64_t* cu_seqlens, int64_t T, int64_t max_seqlen);
+
 int device_sm_count();     // of the CURRENT device (cached per device ordinal)
 
 int current_device();      // cudaGetDevice, -1 on error

@@ -25,9 +25,7 @@
 #include "common.cuh"
 #include "../../include/evo_b200.h"
 #include <algorithm>
-#include "hyena_tma.cuh"
 #include "hyena_ms.cuh"
-#include <stdlib.h>
 
 using namespace evo;
 
@@ -226,21 +224,6 @@ __global__ void fir_state_kernel(const bf16* __restrict__ z, const bf16* __restr
   }
 }
 
-// packed sequences: sequence b's last two z rows, zero history before its first row
-__global__ void fir_state_varlen_kernel(const bf16* __restrict__ z, const long long* __restrict__ cu, bf16* __restrict__ out,
-                                        int n_seq, long long T, long long max_len, long long C3) {
-  long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;   // (b, c)
-  if (idx >= (long long)n_seq * C3) return;
-  long long b = idx / C3, c = idx % C3;
-  const long long row0 = min(max(cu[b], 0LL), T);
-  const long long len = min(min(cu[b + 1], T) - row0, max_len);
-#pragma unroll
-  for (int k = 0; k < 2; ++k) {
-    long long t = len - 2 + k;
-    out[idx * 2 + k] = t >= 0 ? z[(row0 + t) * C3 + c] : __float2bfloat16_rn(0.f);
-  }
-}
-
 // decode step (engine.step_fir + step_iir): 8 lanes per (b, channel).  Lane s owns modal state s (its pole, residue
 // and state are one coalesced 8-byte load each); lanes 0..2 run the three FIR channels (x2, x1, v); lane 0 folds the
 // eight residue products in the reference's order (sequential fma chain) and writes y.
@@ -304,7 +287,7 @@ __global__ void __launch_bounds__(256) hyena_step_kernel(const bf16* __restrict_
 }
 
 bool use_tma_path(const evo_hyena_params* p) {
-  return p->D % evo_hy2::CH_PER_CTA == 0 && p->D / p->nheads == 128;
+  return p->D % evo_hy3::CH_PER_CTA == 0 && p->D / p->nheads == 128;
 }
 
 // Sequential-in-L is the efficient form (one HBM pass, no carry pass); split L only when the
@@ -312,7 +295,7 @@ bool use_tma_path(const evo_hyena_params* p) {
 int pick_segments(const evo_hyena_params* p) {
   const long long L = p->L;
   if (p->force_segments > 0) return (int)std::min<long long>(p->force_segments, std::max<long long>(1, L));
-  const int per_cta = use_tma_path(p) ? evo_hy2::CH_PER_CTA : THREADS;
+  const int per_cta = use_tma_path(p) ? evo_hy3::CH_PER_CTA : THREADS;
   long long blocks = (long long)((p->D + per_cta - 1) / per_cta) * p->B;
   int sms = device_sm_count();
   if (blocks * 5 >= sms * 3 || L < 1024) return 1;
@@ -322,13 +305,57 @@ int pick_segments(const evo_hyena_params* p) {
   return (int)std::max<long long>(1, std::min<long long>(std::min<long long>(want, max_by_len), 64));
 }
 
+// workspace: the zero-start end state of every segment of every sequence, (rows, nseg, D, NS, 2) fp32.  One segment needs
+// none, except in a state-only call, which folds the states afterwards.
+size_t seg_state_bytes(int rows, int nseg, int D, bool state_only) {
+  if (nseg <= 1 && !state_only) return 0;
+  return (size_t)rows * nseg * D * NS * 2 * sizeof(float);
+}
+
+// One form of the mode-split scan (A = Args2: batched; Args2V: packed; Args2R: packed with checkpoints), its arguments filled
+// but for the ring depth: the z map (3D columns x rows x batches, one batch of T rows when packed), the shared-memory limit
+// of the form's two kernels, and either the state-only pass or the state pass over the first nseg - 1 segments (the last
+// segment's zero-start state is never needed; skipped when the workspace already holds the states) and the output pass.
+template <typename A>
+int launch_ms_scan(A a, bool state_only, bool reuse_segment_states, cudaStream_t st) {
+  // every name below is qualified: THREADS, for one, is also this file's scalar-kernel block size
+  namespace hy = evo_hy3;
+  constexpr bool VARLEN = !std::is_same<A, hy::Args2>::value, RESUME = std::is_same<A, hy::Args2R>::value;
+  long long rows = a.L;
+  int batches = a.B;
+  if constexpr (VARLEN) { rows = a.T; batches = 1; }
+  int rc;
+  CUtensorMap tmZ;
+  uint64_t dims[3] = {(uint64_t)3 * a.D, (uint64_t)rows, (uint64_t)batches};
+  uint64_t str[2] = {(uint64_t)3 * a.D * 2, (uint64_t)rows * 3 * a.D * 2};
+  uint32_t box[3] = {128, (uint32_t)hy::T2, 1};
+  if ((rc = make_tmap_nd_bf16(&tmZ, a.z, 3, dims, str, box, false))) return rc;
+  static unsigned long long done_s = 0, done_o = 0;      // one mask per kernel: the limit is an attribute of each kernel
+  if ((rc = ensure_dyn_smem(hy::hyena_scan_ms_kernel<true, VARLEN, RESUME>, hy::smem_bytes(hy::STAGES), done_s))) return rc;
+  if ((rc = ensure_dyn_smem(hy::hyena_scan_ms_kernel<false, VARLEN, RESUME>, hy::smem_bytes(hy::STAGES), done_o))) return rc;
+  // ring depth 4 (96 KB): two CTAs can co-reside and hide each other's latency when the grid exceeds the SM count.
+  // An 8-deep ring for single-CTA-per-SM grids was measured and did not help (1.21 vs 1.06-1.13 ms at B=8, L=8193).
+  a.nst = 4;
+  const int SMEM_BYTES = hy::smem_bytes(a.nst);
+  dim3 grid(a.D / hy::CH_PER_CTA, a.B, a.nseg), block(hy::THREADS);
+  if (state_only) {
+    hy::hyena_scan_ms_kernel<true, VARLEN, RESUME><<<grid, block, SMEM_BYTES, st>>>(tmZ, a);
+    return check_launch("hyena_scan<state>");
+  }
+  if (a.nseg > 1 && !reuse_segment_states) {
+    dim3 g2(grid.x, grid.y, a.nseg - 1);
+    hy::hyena_scan_ms_kernel<true, VARLEN, RESUME><<<g2, block, SMEM_BYTES, st>>>(tmZ, a);
+    if ((rc = check_launch("hyena_scan<state>"))) return rc;
+  }
+  hy::hyena_scan_ms_kernel<false, VARLEN, RESUME><<<grid, block, SMEM_BYTES, st>>>(tmZ, a);
+  return check_launch("hyena_scan<out>");
+}
+
 }  // namespace
 
 extern "C" size_t evo_hyena_fwd_workspace(const evo_hyena_params* p) {
   if (p->L <= 0) return 0;
-  int nseg = pick_segments(p);
-  if (nseg <= 1 && !p->state_only) return 0;
-  return (size_t)p->B * nseg * p->D * NS * 2 * sizeof(float);
+  return seg_state_bytes(p->B, pick_segments(p), p->D, p->state_only);
 }
 
 // segment geometry: equal segments, none empty
@@ -352,47 +379,12 @@ extern "C" int evo_hyena_fwd(const evo_hyena_params* p, void* workspace, size_t 
   else EVO_REQUIRE(p->y != nullptr, "evo_hyena_fwd: y is NULL");
   int rc;
   if (use_tma_path(p)) {
-    using namespace evo_hy2;
-    CUtensorMap tmZ;
-    uint64_t dims[3] = {(uint64_t)3 * p->D, (uint64_t)p->L, (uint64_t)p->B};
-    uint64_t str[2] = {(uint64_t)3 * p->D * 2, (uint64_t)p->L * 3 * p->D * 2};
-    uint32_t box[3] = {128, (uint32_t)T2, 1};
-    if ((rc = make_tmap_nd_bf16(&tmZ, p->z, 3, dims, str, box, false))) return rc;
-    Args2 a;
+    evo_hy3::Args2 a = {};
     a.y = (bf16*)p->y; a.z = (const bf16*)p->z;
     a.fir_w = (const bf16*)p->fir_w; a.fir_b = (const bf16*)p->fir_b; a.Dskip = (const bf16*)p->Dskip;
     a.poles = p->poles; a.residues = p->residues; a.halo = (const bf16*)p->halo; a.state_in = p->state_in; a.state_out = p->state_out;
     a.seg_states = (float*)workspace; a.B = p->B; a.D = p->D; a.nseg = nseg; a.L = p->L; a.seg_len = seg_len;
-    static unsigned long long done_s = 0, done_o = 0;
-    if ((rc = ensure_dyn_smem(hyena_scan_tma_kernel<true>, smem_bytes(STAGES), done_s))) return rc;
-    if ((rc = ensure_dyn_smem(hyena_scan_tma_kernel<false>, smem_bytes(STAGES), done_o))) return rc;
-    // 1 (default) = mode-split kernel (hyena_ms.cuh: 8 compute warps, 4 modal states per thread); 0 = round-1 kernel
-    // (4 compute warps, 8 states per thread), kept for A/B timing and as a second implementation that
-    // tests/test_gpu_hyena_paths.py holds to the same oracle bars and compares with this one
-    const char* env_v = getenv("EVO_B200_HYENA_VARIANT");      // read per call: experiments flip it inside one process
-    const int variant = env_v ? atoi(env_v) : 1;
-    static unsigned long long done_ms = 0, done_mo = 0;
-    if ((rc = ensure_dyn_smem(evo_hy3::hyena_scan_ms_kernel<true>, smem_bytes(STAGES), done_ms))) return rc;
-    if ((rc = ensure_dyn_smem(evo_hy3::hyena_scan_ms_kernel<false>, smem_bytes(STAGES), done_mo))) return rc;
-    dim3 grid(p->D / CH_PER_CTA, p->B, nseg), block(variant == 1 ? evo_hy3::THREADS : evo_hy2::THREADS);
-    auto k_state = variant == 1 ? evo_hy3::hyena_scan_ms_kernel<true> : hyena_scan_tma_kernel<true>;
-    auto k_out = variant == 1 ? evo_hy3::hyena_scan_ms_kernel<false> : hyena_scan_tma_kernel<false>;
-    // ring depth 4 (96 KB): two CTAs can co-reside and hide each other's latency when the grid exceeds the SM count.
-    // An 8-deep ring for single-CTA-per-SM grids was measured and did not help (1.21 vs 1.06-1.13 ms at B=8, L=8193).
-    a.nst = 4;
-    const int SMEM_BYTES = smem_bytes(a.nst);
-    if (p->state_only) {
-      k_state<<<grid, block, SMEM_BYTES, st>>>(tmZ, a);
-      if ((rc = check_launch("hyena_scan<state>"))) return rc;
-    } else {
-      if (nseg > 1 && !p->reuse_segment_states) {
-        dim3 g2(grid.x, grid.y, nseg - 1);
-        k_state<<<g2, block, SMEM_BYTES, st>>>(tmZ, a);
-        if ((rc = check_launch("hyena_scan<state>"))) return rc;
-      }
-      k_out<<<grid, block, SMEM_BYTES, st>>>(tmZ, a);
-      if ((rc = check_launch("hyena_scan<out>"))) return rc;
-    }
+    if ((rc = launch_ms_scan(a, p->state_only, p->reuse_segment_states, st))) return rc;
   } else {
     Args a;
     a.z = (const bf16*)p->z; a.y = (bf16*)p->y;
@@ -429,79 +421,8 @@ extern "C" int evo_hyena_fwd(const evo_hyena_params* p, void* workspace, size_t 
   return 0;
 }
 
-// packed sequences: nseg = pick_segments(B = n_seq, L = max_seqlen) and one common seg_len -- on equal lengths exactly the
-// geometry evo_hyena_fwd gives the (n_seq, L) batch, so the two compute the same bits
-static int varlen_geometry(const evo_hyena_varlen_params* p, int& nseg, long long& seg_len) {
-  EVO_REQUIRE(p->S == NS, "evo_hyena_fwd_varlen: state_size %d unsupported (kernel is specialised for %d)", p->S, NS);
-  EVO_REQUIRE(p->nheads > 0 && p->D % p->nheads == 0 && p->D / p->nheads == 128 && p->D % evo_hy2::CH_PER_CTA == 0,
-              "evo_hyena_fwd_varlen: needs head_dim 128 and D %% 256 == 0 (D %d, %d heads)", p->D, p->nheads);
-  EVO_REQUIRE(p->n_seq > 0 && p->n_seq <= 65535, "evo_hyena_fwd_varlen: bad sequence count %d", p->n_seq);
-  EVO_REQUIRE(p->cu_seqlens != nullptr && p->max_seqlen > 0 && p->max_seqlen <= p->T && p->T < (1LL << 31),
-              "evo_hyena_fwd_varlen: needs cu_seqlens and 0 < max_seqlen <= T < 2^31 (max_seqlen %lld, T %lld)", (long long)p->max_seqlen, (long long)p->T);
-  EVO_REQUIRE(p->seg_len >= 0, "evo_hyena_fwd_varlen: negative seg_len");
-  if (p->seg_len > 0) {
-    seg_len = p->seg_len;
-  } else {
-    evo_hyena_params q = {};
-    q.B = p->n_seq; q.L = p->max_seqlen; q.D = p->D; q.nheads = p->nheads;
-    const int n = pick_segments(&q);
-    seg_len = (q.L + n - 1) / n;
-  }
-  nseg = (int)((p->max_seqlen + seg_len - 1) / seg_len);
-  EVO_REQUIRE(nseg <= 65535, "evo_hyena_fwd_varlen: %d segments", nseg);
-  return 0;
-}
-
-extern "C" size_t evo_hyena_fwd_varlen_workspace(const evo_hyena_varlen_params* p) {
-  int nseg; long long seg_len;
-  if (varlen_geometry(p, nseg, seg_len) || nseg <= 1) return 0;
-  return (size_t)p->n_seq * nseg * p->D * NS * 2 * sizeof(float);
-}
-
-extern "C" int evo_hyena_fwd_varlen(const evo_hyena_varlen_params* p, void* workspace, size_t workspace_bytes, void* stream) {
-  int nseg; long long seg_len;
-  int rc;
-  if ((rc = varlen_geometry(p, nseg, seg_len))) return rc;
-  EVO_REQUIRE(p->z != nullptr && p->y != nullptr, "evo_hyena_fwd_varlen: z or y is NULL");
-  const size_t need = evo_hyena_fwd_varlen_workspace(p);
-  EVO_REQUIRE(workspace_bytes >= need && (need == 0 || workspace), "evo_hyena_fwd_varlen: workspace too small (%zu < %zu)", workspace_bytes, need);
-  cudaStream_t st = (cudaStream_t)stream;
-  using namespace evo_hy2;
-  CUtensorMap tmZ;
-  uint64_t dims[3] = {(uint64_t)3 * p->D, (uint64_t)p->T, 1};
-  uint64_t str[2] = {(uint64_t)3 * p->D * 2, (uint64_t)p->T * 3 * p->D * 2};
-  uint32_t box[3] = {128, (uint32_t)T2, 1};
-  if ((rc = make_tmap_nd_bf16(&tmZ, p->z, 3, dims, str, box, false))) return rc;
-  evo_hy3::Args2V a = {};
-  a.y = (bf16*)p->y; a.z = (const bf16*)p->z;
-  a.fir_w = (const bf16*)p->fir_w; a.fir_b = (const bf16*)p->fir_b; a.Dskip = (const bf16*)p->Dskip;
-  a.poles = p->poles; a.residues = p->residues; a.state_out = p->state_out;
-  a.seg_states = (float*)workspace; a.B = p->n_seq; a.D = p->D; a.nseg = nseg; a.L = p->max_seqlen; a.seg_len = seg_len;
-  a.cu_seqlens = (const long long*)p->cu_seqlens; a.T = p->T;
-  a.nst = 4;
-  static unsigned long long done_s = 0, done_o = 0;
-  if ((rc = ensure_dyn_smem(evo_hy3::hyena_scan_ms_kernel<true, true>, smem_bytes(STAGES), done_s))) return rc;
-  if ((rc = ensure_dyn_smem(evo_hy3::hyena_scan_ms_kernel<false, true>, smem_bytes(STAGES), done_o))) return rc;
-  const int SMEM_BYTES = smem_bytes(a.nst);
-  dim3 grid(p->D / CH_PER_CTA, p->n_seq, nseg), block(evo_hy3::THREADS);
-  if (nseg > 1) {
-    dim3 g2(grid.x, grid.y, nseg - 1);
-    evo_hy3::hyena_scan_ms_kernel<true, true><<<g2, block, SMEM_BYTES, st>>>(tmZ, a);
-    if ((rc = check_launch("hyena_scan_varlen<state>"))) return rc;
-  }
-  evo_hy3::hyena_scan_ms_kernel<false, true><<<grid, block, SMEM_BYTES, st>>>(tmZ, a);
-  if ((rc = check_launch("hyena_scan_varlen<out>"))) return rc;
-  if (p->fir_state_out) {
-    long long n = (long long)p->n_seq * 3 * p->D;
-    fir_state_varlen_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>((const bf16*)p->z, (const long long*)p->cu_seqlens, (bf16*)p->fir_state_out,
-                                                                         p->n_seq, p->T, p->max_seqlen, 3LL * p->D);
-    if ((rc = check_launch("fir_state_varlen"))) return rc;
-  }
-  return 0;
-}
-
-// checkpointed / resumed packed sequences: sequence b's last two z rows, with its starting FIR history (halo_table[start_idx[b]])
-// standing in front of row 0 when it is shorter than two rows
+// packed sequences: sequence b's last two z rows; when it is shorter than two rows, the rows in front of row 0 are its starting
+// FIR history (halo_table[start_idx[b]]) or, without start_idx or at start_idx[b] == -1, zero
 __global__ void fir_state_resume_kernel(const bf16* __restrict__ z, const long long* __restrict__ cu, const long long* __restrict__ start_idx,
                                         const bf16* __restrict__ halo_table, long long n_table, bf16* __restrict__ out,
                                         int n_seq, long long T, long long max_len, long long C3) {
@@ -522,19 +443,80 @@ __global__ void fir_state_resume_kernel(const bf16* __restrict__ z, const long l
   }
 }
 
+// packed sequences: nseg = pick_segments(B = n_seq, L = max_seqlen) and one common seg_len -- on equal lengths exactly the
+// geometry evo_hyena_fwd gives the (n_seq, L) batch, so the two compute the same bits.  `what` names the entry point.
+static int varlen_geometry(const evo_hyena_varlen_params* p, const char* what, int& nseg, long long& seg_len) {
+  EVO_REQUIRE(p->S == NS, "%s: state_size %d unsupported (kernel is specialised for %d)", what, p->S, NS);
+  EVO_REQUIRE(p->nheads > 0 && p->D % p->nheads == 0 && p->D / p->nheads == 128 && p->D % evo_hy3::CH_PER_CTA == 0,
+              "%s: needs head_dim 128 and D %% 256 == 0 (D %d, %d heads)", what, p->D, p->nheads);
+  EVO_REQUIRE(p->n_seq > 0 && p->n_seq <= 65535, "%s: bad sequence count %d", what, p->n_seq);
+  int rc;
+  if ((rc = check_packed(what, p->cu_seqlens, p->T, p->max_seqlen))) return rc;
+  EVO_REQUIRE(p->seg_len >= 0, "%s: negative seg_len", what);
+  if (p->seg_len > 0) {
+    seg_len = p->seg_len;
+  } else {
+    evo_hyena_params q = {};
+    q.B = p->n_seq; q.L = p->max_seqlen; q.D = p->D; q.nheads = p->nheads;
+    const int n = pick_segments(&q);
+    seg_len = (q.L + n - 1) / n;
+  }
+  nseg = (int)((p->max_seqlen + seg_len - 1) / seg_len);
+  EVO_REQUIRE(nseg <= 65535, "%s: %d segments", what, nseg);
+  return 0;
+}
+
+// the scan arguments every packed call shares; the checkpointed form adds its own on top
+static void fill_varlen_args(evo_hy3::Args2V& a, const evo_hyena_varlen_params* p, void* workspace, int nseg, long long seg_len) {
+  a.y = (bf16*)p->y; a.z = (const bf16*)p->z;
+  a.fir_w = (const bf16*)p->fir_w; a.fir_b = (const bf16*)p->fir_b; a.Dskip = (const bf16*)p->Dskip;
+  a.poles = p->poles; a.residues = p->residues; a.state_out = p->state_out;
+  a.seg_states = (float*)workspace; a.B = p->n_seq; a.D = p->D; a.nseg = nseg; a.L = p->max_seqlen; a.seg_len = seg_len;
+  a.cu_seqlens = (const long long*)p->cu_seqlens; a.T = p->T;
+}
+
+// fir_state_out of a packed call (start_idx NULL: every sequence starts from zero history)
+static int fir_state_packed(const evo_hyena_varlen_params* p, const long long* start_idx, const bf16* halo_table, long long n_table, cudaStream_t st) {
+  if (!p->fir_state_out) return 0;
+  long long n = (long long)p->n_seq * 3 * p->D;
+  fir_state_resume_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>((const bf16*)p->z, (const long long*)p->cu_seqlens, start_idx, halo_table,
+                                                                       n_table, (bf16*)p->fir_state_out, p->n_seq, p->T, p->max_seqlen, 3LL * p->D);
+  return check_launch("fir_state_resume");
+}
+
+extern "C" size_t evo_hyena_fwd_varlen_workspace(const evo_hyena_varlen_params* p) {
+  int nseg; long long seg_len;
+  if (varlen_geometry(p, "evo_hyena_fwd_varlen", nseg, seg_len)) return 0;
+  return seg_state_bytes(p->n_seq, nseg, p->D, false);
+}
+
+extern "C" int evo_hyena_fwd_varlen(const evo_hyena_varlen_params* p, void* workspace, size_t workspace_bytes, void* stream) {
+  int nseg; long long seg_len;
+  int rc;
+  if ((rc = varlen_geometry(p, "evo_hyena_fwd_varlen", nseg, seg_len))) return rc;
+  EVO_REQUIRE(p->z != nullptr && p->y != nullptr, "evo_hyena_fwd_varlen: z or y is NULL");
+  const size_t need = seg_state_bytes(p->n_seq, nseg, p->D, false);
+  EVO_REQUIRE(workspace_bytes >= need && (need == 0 || workspace), "evo_hyena_fwd_varlen: workspace too small (%zu < %zu)", workspace_bytes, need);
+  cudaStream_t st = (cudaStream_t)stream;
+  evo_hy3::Args2V a = {};
+  fill_varlen_args(a, p, workspace, nseg, seg_len);
+  if ((rc = launch_ms_scan(a, false, false, st))) return rc;
+  return fir_state_packed(p, nullptr, nullptr, 0, st);
+}
+
 // The checkpointed form keeps every segment start on the 16-token stage, so that each checkpoint ends a full tile
 static int ckpt_geometry(const evo_hyena_varlen_ckpt_params* p, int& nseg, long long& seg_len) {
   int rc;
-  if ((rc = varlen_geometry(&p->base, nseg, seg_len))) return rc;
+  if ((rc = varlen_geometry(&p->base, "evo_hyena_fwd_varlen_ckpt", nseg, seg_len))) return rc;
   if (p->ckpt_states) {
     EVO_REQUIRE(p->ckpt_stride > 0 && p->ckpt_stride % 128 == 0 && p->ckpt_base != nullptr && p->n_ckpt > 0,
                 "evo_hyena_fwd_varlen_ckpt: checkpoints need ckpt_base, n_ckpt > 0 and a stride that is a positive multiple of 128 (got %lld)",
                 (long long)p->ckpt_stride);
     if (p->base.seg_len > 0) {
-      EVO_REQUIRE(seg_len % evo_hy2::T2 == 0, "evo_hyena_fwd_varlen_ckpt: with checkpoints a forced seg_len must be a multiple of %d (got %lld)",
-                  evo_hy2::T2, seg_len);
+      EVO_REQUIRE(seg_len % evo_hy3::T2 == 0, "evo_hyena_fwd_varlen_ckpt: with checkpoints a forced seg_len must be a multiple of %d (got %lld)",
+                  evo_hy3::T2, seg_len);
     } else {
-      seg_len = (seg_len + evo_hy2::T2 - 1) / evo_hy2::T2 * evo_hy2::T2;
+      seg_len = (seg_len + evo_hy3::T2 - 1) / evo_hy3::T2 * evo_hy3::T2;
       nseg = (int)((p->base.max_seqlen + seg_len - 1) / seg_len);
     }
   }
@@ -545,8 +527,8 @@ static int ckpt_geometry(const evo_hyena_varlen_ckpt_params* p, int& nseg, long 
 
 extern "C" size_t evo_hyena_fwd_varlen_ckpt_workspace(const evo_hyena_varlen_ckpt_params* p) {
   int nseg; long long seg_len;
-  if (ckpt_geometry(p, nseg, seg_len) || nseg <= 1) return 0;
-  return (size_t)p->base.n_seq * nseg * p->base.D * NS * 2 * sizeof(float);
+  if (ckpt_geometry(p, nseg, seg_len)) return 0;
+  return seg_state_bytes(p->base.n_seq, nseg, p->base.D, false);
 }
 
 extern "C" int evo_hyena_fwd_varlen_ckpt(const evo_hyena_varlen_ckpt_params* p, void* workspace, size_t workspace_bytes, void* stream) {
@@ -555,43 +537,15 @@ extern "C" int evo_hyena_fwd_varlen_ckpt(const evo_hyena_varlen_ckpt_params* p, 
   if ((rc = ckpt_geometry(p, nseg, seg_len))) return rc;
   const evo_hyena_varlen_params* q = &p->base;
   EVO_REQUIRE(q->z != nullptr && q->y != nullptr, "evo_hyena_fwd_varlen_ckpt: z or y is NULL");
-  const size_t need = evo_hyena_fwd_varlen_ckpt_workspace(p);
+  const size_t need = seg_state_bytes(q->n_seq, nseg, q->D, false);
   EVO_REQUIRE(workspace_bytes >= need && (need == 0 || workspace), "evo_hyena_fwd_varlen_ckpt: workspace too small (%zu < %zu)", workspace_bytes, need);
   cudaStream_t st = (cudaStream_t)stream;
-  using namespace evo_hy2;
-  CUtensorMap tmZ;
-  uint64_t dims[3] = {(uint64_t)3 * q->D, (uint64_t)q->T, 1};
-  uint64_t str[2] = {(uint64_t)3 * q->D * 2, (uint64_t)q->T * 3 * q->D * 2};
-  uint32_t box[3] = {128, (uint32_t)T2, 1};
-  if ((rc = make_tmap_nd_bf16(&tmZ, q->z, 3, dims, str, box, false))) return rc;
   evo_hy3::Args2R a = {};
-  a.y = (bf16*)q->y; a.z = (const bf16*)q->z;
-  a.fir_w = (const bf16*)q->fir_w; a.fir_b = (const bf16*)q->fir_b; a.Dskip = (const bf16*)q->Dskip;
-  a.poles = q->poles; a.residues = q->residues; a.state_out = q->state_out;
-  a.seg_states = (float*)workspace; a.B = q->n_seq; a.D = q->D; a.nseg = nseg; a.L = q->max_seqlen; a.seg_len = seg_len;
-  a.cu_seqlens = (const long long*)q->cu_seqlens; a.T = q->T;
+  fill_varlen_args(a, q, workspace, nseg, seg_len);
   a.ckpt_out = p->ckpt_states; a.ckpt_base = (const long long*)p->ckpt_base; a.ckpt_stride = p->ckpt_stride; a.n_ckpt = p->n_ckpt;
   a.start_idx = (const long long*)p->start_idx; a.state_table = p->state_table; a.halo_table = (const bf16*)p->halo_table; a.n_table = p->n_table;
-  a.nst = 4;
-  static unsigned long long done_s = 0, done_o = 0;
-  if ((rc = ensure_dyn_smem(evo_hy3::hyena_scan_ms_kernel<true, true, true>, smem_bytes(STAGES), done_s))) return rc;
-  if ((rc = ensure_dyn_smem(evo_hy3::hyena_scan_ms_kernel<false, true, true>, smem_bytes(STAGES), done_o))) return rc;
-  const int SMEM_BYTES = smem_bytes(a.nst);
-  dim3 grid(q->D / CH_PER_CTA, q->n_seq, nseg), block(evo_hy3::THREADS);
-  if (nseg > 1) {
-    dim3 g2(grid.x, grid.y, nseg - 1);
-    evo_hy3::hyena_scan_ms_kernel<true, true, true><<<g2, block, SMEM_BYTES, st>>>(tmZ, a);
-    if ((rc = check_launch("hyena_scan_varlen_ckpt<state>"))) return rc;
-  }
-  evo_hy3::hyena_scan_ms_kernel<false, true, true><<<grid, block, SMEM_BYTES, st>>>(tmZ, a);
-  if ((rc = check_launch("hyena_scan_varlen_ckpt<out>"))) return rc;
-  if (q->fir_state_out) {
-    long long n = (long long)q->n_seq * 3 * q->D;
-    fir_state_resume_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>((const bf16*)q->z, (const long long*)q->cu_seqlens, a.start_idx, a.halo_table,
-                                                                         a.n_table, (bf16*)q->fir_state_out, q->n_seq, q->T, q->max_seqlen, 3LL * q->D);
-    if ((rc = check_launch("fir_state_resume"))) return rc;
-  }
-  return 0;
+  if ((rc = launch_ms_scan(a, false, false, st))) return rc;
+  return fir_state_packed(q, a.start_idx, a.halo_table, a.n_table, st);
 }
 
 extern "C" int evo_hyena_step(const void* u, void* y, void* fir_state, float* state,

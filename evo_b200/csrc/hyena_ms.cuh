@@ -1,12 +1,13 @@
-// Hyena scan, mode-split variant (round 2): the production path for head_dim 128 / D % 256 == 0.
+// Hyena scan, mode-split TMA kernel: the production path for head_dim 128 / D % 256 == 0.
 //
-// Same operator, same rounding points and the same TMA ring as hyena_scan_tma_kernel (hyena_tma.cuh); what changes
-// is the work assignment, because that kernel is latency-starved, not bandwidth- or pipe-bound: 128 CTAs x 4
-// compute warps = ONE warp per SM sub-partition and 214 registers per thread.  Here
-//   * a thread still carries a channel PAIR (fp32 pair arithmetic, fadd2 / fmul2 / ffma2), but only FOUR of the
-//     eight modal states: lanes l and l^16 of a warp share a pair.
-//     Registers per thread drop to ~half and a 256-channel CTA has 8 compute warps = two per sub-partition, so a
-//     dependent FMA chain in one warp is covered by the other;
+// Same operator and rounding points as hyena_scan_kernel (hyena.cu); what changes is how the machine is driven:
+//   * a CTA owns two heads (256 channels) of one batch row and walks its L segment in tiles of T2 tokens; a producer
+//     warp keeps an mbarrier ring of z tiles ([x2|x1|v] x 2 heads = six 128-column boxes, 24 KB per stage) in flight
+//     by TMA, so HBM latency is never exposed to the scan;
+//   * a thread carries a channel PAIR (fp32 pair arithmetic, fadd2 / fmul2 / ffma2, one rounding per lane), but only
+//     FOUR of the eight modal states: lanes l and l^16 of a warp share a pair.  A thread that carried all eight states
+//     needed ~214 registers and left one warp per SM sub-partition, latency-starved; here a 256-channel CTA has
+//     8 compute warps = two per sub-partition, so a dependent FMA chain in one warp is covered by the other;
 //   * the element-wise work is split between the two halves instead of duplicated: half 0 runs the x1 FIR, half 1
 //     the v FIR (one shuffle exchanges the bf16x2 results); half 0 gates tokens 0..3 of a group of eight, half 1
 //     tokens 4..7 (one shuffle per fp32 word moves the partial residue sums to the half that needs them);
@@ -14,44 +15,64 @@
 //     add.rn.bf16x2 / mul.rn.bf16x2 instead of unpack + fp32 op + pack: the product of two bf16 is exact in fp32 and
 //     the sum of two bf16 is exact in fp32 or rounds to the larger operand either way, so a single rounding of the
 //     exact result is bit-identical to the reference's "compute in fp32, round to bf16".
-// fma-pipe instructions per token per channel pair: 68 (was 67); ALU conversions ~21 (was ~38).
 #pragma once
-#include "hyena_tma.cuh"
+#include "common.cuh"
 #include <type_traits>
 
 namespace evo_hy3 {
 
 using namespace evo;
-using evo_hy2::Args2;
-using evo_hy2::C2;
-using evo_hy2::cmul2;
-using evo_hy2::cpow2;
-using evo_hy2::lds32;
-using evo_hy2::unpack2;
 
 constexpr int NS = 8;
 constexpr int NSH = 4;                       // modal states per thread
-constexpr int T2 = evo_hy2::T2;              // tokens per stage
-constexpr int STAGES = evo_hy2::STAGES;
-constexpr int CH_PER_CTA = 256;
-constexpr int SUB_BYTES = evo_hy2::SUB_BYTES;
-constexpr int STAGE_BYTES = evo_hy2::STAGE_BYTES;
+constexpr int T2 = 16;                       // tokens per stage
+constexpr int STAGES = 8;                    // maximum ring depth (barriers); the launch uses 4
+constexpr int CH_PER_CTA = 256;              // two heads of 128
+constexpr int SUB_BYTES = T2 * 128 * 2;      // one 128-column box
+constexpr int STAGE_BYTES = 6 * SUB_BYTES;   // [head0: x2 x1 v][head1: x2 x1 v]
 constexpr int CWARPS = 8;                    // compute warps: 4 per head, 16 channel pairs x 2 halves each
 constexpr int THREADS = (CWARPS + 1) * 32;   // + 1 TMA producer warp
 constexpr int G = 8;                         // tokens per group
-constexpr int smem_bytes(int nst) { return evo_hy2::smem_bytes(nst); }
+constexpr int smem_bytes(int nst) { return nst * STAGE_BYTES + 128 + 1024; }
 
-struct Args2V : Args2 {                      // packed sequences (VARLEN); Args2 itself stays as it is, and so do its kernels
+struct Args2 {                               // batched sequences
+  bf16* y;
+  const bf16* z;
+  const bf16* fir_w; const bf16* fir_b; const bf16* Dskip;
+  const float* poles; const float* residues;
+  const bf16* halo; const float* state_in;
+  float* state_out;
+  float* seg_states;                         // (B, nseg, D, NS, 2) zero-start end states of each segment
+  int B, D, nseg, nst;
+  long long L, seg_len;
+};
+struct Args2V : Args2 {                      // packed sequences (VARLEN)
   const long long* cu_seqlens;               // (B + 1) row offsets; Args2::L is the longest length
   long long T;                               // packed rows
 };
-struct Args2R : Args2V {                     // checkpoint emission and resumed starts (RESUME); Args2V and its kernels stay as they are
+struct Args2R : Args2V {                     // checkpoint emission and resumed starts (RESUME)
   // emission: the output pass stores the running state after row k*ckpt_stride - 1 of sequence b at table row ckpt_base[b] + k - 1
   // (k >= 1, k*ckpt_stride < its length; ckpt_stride a multiple of 128, seg_len a multiple of the 16-token stage), NULL = none
   float* ckpt_out; const long long* ckpt_base; long long ckpt_stride, n_ckpt;
   // resumed start: sequence b starts from state_table[start_idx[b]] and FIR history halo_table[start_idx[b]] (-1 = zero start)
   const long long* start_idx; const float* state_table; const bf16* halo_table; long long n_table;
 };
+
+__device__ __forceinline__ float2 unpack2(uint32_t v) { return make_float2(bf_lo(v), bf_hi(v)); }
+__device__ __forceinline__ uint32_t lds32(uint32_t addr) { uint32_t v; asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr)); return v; }
+
+struct C2 { float2 r, i; };                  // two complex numbers (one per channel of the pair)
+__device__ __forceinline__ C2 cmul2(C2 a, C2 b) {
+  C2 o;
+  o.r = ffma2(a.r, b.r, fmul2(make_float2(-a.i.x, -a.i.y), b.i));
+  o.i = ffma2(a.r, b.i, fmul2(a.i, b.r));
+  return o;
+}
+__device__ __forceinline__ C2 cpow2(C2 p, long long n) {
+  C2 acc; acc.r = make_float2(1.f, 1.f); acc.i = make_float2(0.f, 0.f);
+  while (n > 0) { if (n & 1) acc = cmul2(acc, p); p = cmul2(p, p); n >>= 1; }
+  return acc;
+}
 
 __device__ __forceinline__ uint32_t mul_bf2(uint32_t a, uint32_t b) { uint32_t d; asm("mul.rn.bf16x2 %0, %1, %2;" : "=r"(d) : "r"(a), "r"(b)); return d; }
 __device__ __forceinline__ uint32_t add_bf2(uint32_t a, uint32_t b) { uint32_t d; asm("add.rn.bf16x2 %0, %1, %2;" : "=r"(d) : "r"(a), "r"(b)); return d; }

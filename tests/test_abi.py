@@ -113,3 +113,47 @@ def test_error_convention_without_a_gpu():
         _lib.check(lib.evo_kv_append(None, None, 1, 10, 2, 128, 10, 16, None), "evo_kv_append")
     rc = lib.evo_rmsnorm(ctypes.c_void_p(0x1000), ctypes.c_void_p(0x2000), ctypes.c_void_p(0x3000), 4, 4096, 1e-6, None)
     assert rc < 0 and b"failed" in lib.evo_last_error()
+
+    # packed forms: bad geometry is rejected with its reason before anything touches the device (a workspace query answers 0)
+    def hyena(**kw):
+        f = dict(z=0x1000, y=0x2000, cu_seqlens=0x3000, n_seq=1, T=256, max_seqlen=256, D=256, S=8, nheads=2)
+        f.update(kw)
+        return _lib.HyenaVarlenParams(**f)
+
+    def rejected(rc, msg):
+        return rc < 0 and msg in lib.evo_last_error()
+
+    def ws_rejected(n, msg):
+        return n == 0 and msg in lib.evo_last_error()
+
+    no_cu = b"needs cu_seqlens and 0 < max_seqlen <= T < 2^31"
+    p = hyena(cu_seqlens=None)
+    assert rejected(lib.evo_hyena_fwd_varlen(ctypes.byref(p), None, 0, None), no_cu)
+    p = hyena(max_seqlen=300)
+    assert ws_rejected(lib.evo_hyena_fwd_varlen_workspace(ctypes.byref(p)), b"(max_seqlen 300, T 256)")
+    p = hyena(nheads=4)
+    assert rejected(lib.evo_hyena_fwd_varlen(ctypes.byref(p), None, 0, None), b"needs head_dim 128 and D % 256 == 0 (D 256, 4 heads)")
+    c = _lib.HyenaVarlenCkptParams(base=hyena(cu_seqlens=None))
+    assert rejected(lib.evo_hyena_fwd_varlen_ckpt(ctypes.byref(c), None, 0, None), no_cu)
+    c = _lib.HyenaVarlenCkptParams(base=hyena(max_seqlen=301))
+    assert ws_rejected(lib.evo_hyena_fwd_varlen_ckpt_workspace(ctypes.byref(c)), b"(max_seqlen 301, T 256)")
+    c = _lib.HyenaVarlenCkptParams(base=hyena(), ckpt_states=0x4000, ckpt_base=0x5000, ckpt_stride=100, n_ckpt=4)
+    assert rejected(lib.evo_hyena_fwd_varlen_ckpt(ctypes.byref(c), None, 0, None),
+                    b"evo_hyena_fwd_varlen_ckpt: checkpoints need ckpt_base, n_ckpt > 0 and a stride that is a positive multiple of 128 (got 100)")
+    c.ckpt_stride = 228
+    assert ws_rejected(lib.evo_hyena_fwd_varlen_ckpt_workspace(ctypes.byref(c)), b"multiple of 128 (got 228)")
+
+    a = _lib.AttnVarlenParams(q=0x1000, k=0x2000, v=0x3000, out=0x4000, q_tok_stride=384, kv_tok_stride=384, cu_seqlens=None, n_seq=1,
+                              T=256, max_seqlen=256, H=1, hd=128, softmax_scale=0.088)
+    assert rejected(lib.evo_attn_fwd_varlen(ctypes.byref(a), None), b"evo_attn_fwd_varlen: " + no_cu)
+    a.cu_seqlens, a.max_seqlen = 0x5000, 257
+    assert rejected(lib.evo_attn_fwd_varlen(ctypes.byref(a), None), b"(max_seqlen 257, T 256)")
+    a.max_seqlen, a.hd = 256, 64
+    assert rejected(lib.evo_attn_fwd_varlen(ctypes.byref(a), None), b"evo_attn_fwd_varlen: head_dim 64 unsupported")
+    a = _lib.AttnVarlenPrefixParams(qkv=0x1000, out=0x2000, cu_seqlens=0x3000, n_seq=1, T=256, max_seqlen=256, cache=None, n_cache=1,
+                                    cache_len=256, prefix_seq=0x4000, prefix_len=0x5000, H=1, hd=128, softmax_scale=0.088)
+    assert rejected(lib.evo_attn_fwd_varlen_prefix(ctypes.byref(a), None), b"evo_attn_fwd_varlen_prefix: needs a cache")
+    a.cu_seqlens = None
+    assert rejected(lib.evo_attn_fwd_varlen_prefix(ctypes.byref(a), None), b"evo_attn_fwd_varlen_prefix: " + no_cu)
+    a.cu_seqlens, a.hd = 0x3000, 96
+    assert rejected(lib.evo_attn_fwd_varlen_prefix(ctypes.byref(a), None), b"evo_attn_fwd_varlen_prefix: head_dim 96 unsupported")

@@ -1,12 +1,12 @@
 """Every implementation and mode of the Hyena operator against the oracle.
 
-evo_hyena_fwd has three scan kernels: the mode-split TMA kernel (hyena_ms.cuh, the default), the round-1 TMA kernel
-(hyena_tma.cuh, EVO_B200_HYENA_VARIANT=0), both taken when head_dim == 128 and D % 256 == 0, and the scalar kernel
-(hyena_scan_kernel in hyena.cu) for every other geometry.  All three claim the reference's bf16 rounding points, so all
-three are held to the bars of tests/test_gpu_parity.py::test_hyena_operator_vs_oracle.  On top of the plain prefill this
-file covers the history inputs (halo, state_in), the carry passes the sequence-parallel forward chains (state_only with
-its fold kernel, evo_hyena_combine_states, reuse_segment_states), the decode step at the 7B width and at head_dim != 128,
-the decode step fused into the in-projection's epilogue, and the calls the launcher must reject.
+evo_hyena_fwd has two scan kernels: the mode-split TMA kernel (hyena_ms.cuh), taken when head_dim == 128 and
+D % 256 == 0, and the scalar kernel (hyena_scan_kernel in hyena.cu) for every other geometry.  Both claim the
+reference's bf16 rounding points, so both are held to the bars of
+tests/test_gpu_parity.py::test_hyena_operator_vs_oracle.  On top of the plain prefill this file covers the history
+inputs (halo, state_in), the carry passes the sequence-parallel forward chains (state_only with its fold kernel,
+evo_hyena_combine_states, reuse_segment_states), the decode step at the 7B width and at head_dim != 128, the decode step
+fused into the in-projection's epilogue, and the calls the launcher must reject.
 
 References: the oracle's bf16 FFT operator (the reference's rounding points) and the fp64 time-domain recurrence
 O.hyena_operator_time_domain (the truth; it takes a halo and a modal state).  Where the FFT operator cannot express an
@@ -32,11 +32,10 @@ from evo_b200 import _lib                             # noqa: E402
 
 DEV = "cuda:0"
 BF16_EPS = 2.0 ** -7
-VARIANT = "EVO_B200_HYENA_VARIANT"
 
-# implementation -> (D, heads, EVO_B200_HYENA_VARIANT).  The scalar kernel is selected by geometry: head_dim 64, and
-# head_dim 128 with D % 256 != 0.
-IMPLS = {"ms": (256, 2, "1"), "tma0": (256, 2, "0"), "scalar_hd64": (256, 4, "1"), "scalar_d384": (384, 3, "1")}
+# implementation -> (D, heads).  The kernel is selected by geometry: the scalar kernel runs head_dim 64, and head_dim 128
+# with D % 256 != 0.
+IMPLS = {"ms": (256, 2), "scalar_hd64": (256, 4), "scalar_d384": (384, 3)}
 LENGTHS = (1, 2, 3, 15, 16, 17, 130, 1025, 4099)      # 16-token TMA stage, 8-token group, ragged last tiles
 FORCES = (0, 1, 3, 7)                                 # 0 = the launcher's choice (8 x 513 tokens at B = 1, L = 4099)
 PREFIX = 37                                           # rows before z in the continuation checks
@@ -169,7 +168,7 @@ def _matrix():
 
 @lru_cache(maxsize=2)
 def _prefill_refs(D, H, B, L):
-    """Inputs and the GPU-independent references of one (geometry, B, L) cell; the two TMA kernels share them."""
+    """Inputs and the GPU-independent references of one (geometry, B, L) cell."""
     sd, _ = _filter_sd(D)
     g = torch.Generator().manual_seed(7919 * L + B)
     z = torch.randn(B, L, 3 * D, generator=g).bfloat16()
@@ -189,12 +188,11 @@ def _prefill_refs(D, H, B, L):
 
 
 @pytest.mark.parametrize("impl,B,L", _matrix())
-def test_prefill_scan_matrix(impl, B, L, monkeypatch):
+def test_prefill_scan_matrix(impl, B, L):
     """One implementation at one (B, L), every segment count (auto, 1, 3, 7: segments shorter than a group, lengths that
     are no multiple of 16, more segments than tokens) and every mode: plain; state_out + fir_state_out; halo; state_in;
     halo + state_in."""
-    D, H, variant = IMPLS[impl]
-    monkeypatch.setenv(VARIANT, variant)
+    D, H = IMPLS[impl]
     sd, f = _filter_sd(D)
     o = _prefill_refs(D, H, B, L)
     z, halo = o.z.to(DEV), o.halo.to(DEV)
@@ -241,8 +239,8 @@ def test_prefill_scan_matrix(impl, B, L, monkeypatch):
 
 
 @pytest.mark.parametrize("B,L", [pytest.param(B, L, id=f"B{B}-L{L}") for B in (1, 3) for L in LENGTHS])
-def test_prefill_implementations_agree(B, L, monkeypatch):
-    """The three kernels on the same two heads: the TMA kernels at D = 256, the scalar kernel as heads 0-1 of D = 384 (whose
+def test_prefill_implementations_agree(B, L):
+    """The two kernels on the same two heads: the TMA kernel at D = 256, the scalar kernel as heads 0-1 of D = 384 (whose
     first 768 z columns and 256 channels are the D = 256 problem).  They differ only in the fp32 order of the residue sum."""
     _, f256 = _filter_sd(256)
     _, f384 = _filter_sd(384)
@@ -250,13 +248,9 @@ def test_prefill_implementations_agree(B, L, monkeypatch):
     z = torch.randn(B, L, 3 * 384, device=DEV).bfloat16()
     z256 = z[..., :768].contiguous()
     for force in FORCES:
-        out = {}
-        for impl in ("ms", "tma0"):
-            monkeypatch.setenv(VARIANT, IMPLS[impl][2])
-            out[impl] = _hyena_call(z256, f256, 2, force=force)[0]
-        out["scalar"] = _hyena_call(z, f384, 3, force=force)[0][..., :256]
-        for a, b in (("ms", "tma0"), ("ms", "scalar"), ("tma0", "scalar")):
-            _assert_same_bf16(out[a], out[b], f"{a} vs {b} B={B} L={L} force={force}", 0.995)
+        ms = _hyena_call(z256, f256, 2, force=force)[0]
+        scalar = _hyena_call(z, f384, 3, force=force)[0][..., :256]
+        _assert_same_bf16(ms, scalar, f"ms vs scalar B={B} L={L} force={force}", 0.995)
 
 
 # ------------------------------------------------------------------ B. carry passes
@@ -270,12 +264,11 @@ def _carry_inputs(D, B, L, seed):
 
 @pytest.mark.parametrize("nseg", [1, 3, 8])
 @pytest.mark.parametrize("impl", list(IMPLS))
-def test_state_only_pass_and_fold(impl, nseg, monkeypatch):
+def test_state_only_pass_and_fold(impl, nseg):
     """state_only: per-segment zero-start end states, folded by hyena_fold_states_kernel (3 segments: 334 + 334 + 333
     tokens; 8 segments: 7 x 126 + 119), with and without halo and state_in, against the fp64 end state and against the
     end state of an output pass at the same geometry."""
-    D, H, variant = IMPLS[impl]
-    monkeypatch.setenv(VARIANT, variant)
+    D, H = IMPLS[impl]
     sd, f = _filter_sd(D, seed=2, pole_mag=NEAR_UNIT)
     B, L = 2, 1001
     z, halo, s_in = _carry_inputs(D, B, L, seed=nseg)
@@ -294,12 +287,11 @@ def test_state_only_pass_and_fold(impl, nseg, monkeypatch):
 
 @pytest.mark.parametrize("force", [0, 3, 8])
 @pytest.mark.parametrize("impl", list(IMPLS))
-def test_output_pass_reusing_carry_states_is_bit_identical(impl, force, monkeypatch):
+def test_output_pass_reusing_carry_states_is_bit_identical(impl, force):
     """state_only, then an output pass with reuse_segment_states = 1 on the same workspace (the order of
     evo_b200/parallel.py): the state kernel computes the same segment states as inside a plain output pass, so y and the
     end state are bit-identical to it.  A zeroed workspace must change y: the flag really reads the kept states."""
-    D, H, variant = IMPLS[impl]
-    monkeypatch.setenv(VARIANT, variant)
+    D, H = IMPLS[impl]
     _, f = _filter_sd(D, seed=2, pole_mag=NEAR_UNIT)
     B, L = 1, 4099
     z, halo, s_in = (t.to(DEV) for t in _carry_inputs(D, B, L, seed=force))
