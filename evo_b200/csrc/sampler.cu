@@ -4,12 +4,13 @@
 // (evo/generation.py:131-189: pick token, store logits/token, feed the token back): greedy when top_k == 1, else
 // top-k -> / temperature -> top-p tail mask -> multinomial, 512-way per row.  The reference draws from torch's
 // global RNG, so only the greedy path can be bit-identical; the sampling path reproduces the DISTRIBUTION
-// (tests/test_gpu_parity.py checks the kept set and a chi-square of the draws against the host implementation) with
-// a counter-based Philox4x32-10 stream keyed by (seed, step, row), which makes a generation reproducible under
-// CUDA-graph replay (no host RNG state inside the loop).
+// (tests/test_gpu_generation.py checks the kept set and a total-variation bound on the draws against the host
+// implementation) with a counter-based Philox4x32-10 stream keyed by (seed, step, row), which makes a generation
+// reproducible under CUDA-graph replay (no host RNG state inside the loop).
 //
 // One CTA per row, one thread per vocabulary entry (V <= 1024):
-//   rank of every entry by counting (V^2 broadcast compares from shared memory; stable: ties -> lower index first),
+//   rank of every entry by counting (V^2 broadcast compares from shared memory; stable: ties -> lower index first;
+//   NaN logits take the last ranks, in index order, and weigh nothing: a NaN is picked only when the whole row is NaN),
 //   top-k = ranks < k, bf16-rounded temperature division like the reference's bf16 tensor op, softmax over the kept
 //   set, suffix sums (Hillis-Steele) for the "cumulative mass from the smallest up" top-p mask, inverse-CDF draw.
 #include "common.cuh"
@@ -51,13 +52,21 @@ __device__ int sample_row(const bf16* __restrict__ logits, int V, const SampleCf
   s_val[t] = mine;
   __syncthreads();
   // stable descending rank: entries strictly greater, or equal with a lower index, come first (argmax = rank 0 = first maximum)
+  // A NaN compares false with everything, so finite entries take ranks [0, nfinite) among themselves; each NaN ranks after
+  // every finite entry and after the NaNs of lower index, which makes the ranks a permutation of [0, V).
   int rank = 0;
   if (t < V) {
-    for (int j = 0; j < V; ++j) {
-      const float o = s_val[j];
-      rank += (o > mine) || (o == mine && j < t);
+    if (mine == mine) {
+      for (int j = 0; j < V; ++j) {
+        const float o = s_val[j];
+        rank += (o > mine) || (o == mine && j < t);
+      }
+    } else {
+      for (int j = 0; j < V; ++j) {
+        const float o = s_val[j];
+        rank += (o == o) || j < t;
+      }
     }
-    if (mine != mine) rank = V - 1;    // NaN logits sort last (never picked unless everything is NaN)
   }
   __syncthreads();
   if (cfg.top_k == 1) {
@@ -75,8 +84,8 @@ __device__ int sample_row(const bf16* __restrict__ logits, int V, const SampleCf
   const float v = kept ? s_scan[0][t] : -INFINITY;       // thread t now owns RANK t
   const float vmax = s_scan[0][0];
   __syncthreads();
-  // softmax over the kept set
-  float e = kept ? __expf(v - vmax) : 0.f;
+  // softmax over the kept set; a NaN weighs nothing (vmax is NaN only when every entry is, and then nothing weighs)
+  float e = (kept && v == v) ? __expf(v - vmax) : 0.f;
   float sum = e;
 #pragma unroll
   for (int off = 16; off > 0; off >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, off);
