@@ -12,7 +12,6 @@ LIB_PATH = os.path.join(_HERE, "libevo_b200.so")
 
 EPI_NONE, EPI_BIAS, EPI_BIAS_RESID, EPI_RESID, EPI_GELU_GATE = range(5)
 EPI_BIAS_ROPE = 6
-EPI_HYENA_STEP = 7
 
 
 class EvoError(RuntimeError):
@@ -31,9 +30,7 @@ class GemmSmallMParams(C.Structure):
     _fields_ = [("A", C.c_void_p), ("lda", C.c_int64), ("W", C.c_void_p), ("C", C.c_void_p), ("ldc", C.c_int64),
                 ("bias", C.c_void_p), ("residual", C.c_void_p), ("ldr", C.c_int64),
                 ("M", C.c_int64), ("N", C.c_int64), ("K", C.c_int64), ("epilogue", C.c_int),
-                ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t),
-                ("fir_state", C.c_void_p), ("state", C.c_void_p), ("fir_w", C.c_void_p), ("fir_b", C.c_void_p), ("Dskip", C.c_void_p),
-                ("poles", C.c_void_p), ("residues", C.c_void_p)]
+                ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t)]
 
 
 class HyenaParams(C.Structure):
@@ -140,7 +137,6 @@ SIGNATURES = {
     "evo_decode_qkv_prep": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int64, C.c_void_p]),
     "evo_decode_attn_workspace": (C.c_size_t, [C.c_int, C.c_int, C.c_int]),
     "evo_decode_attn": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int64, C.c_int, C.c_float, C.c_void_p, C.c_size_t, C.c_void_p]),
-    "evo_advance_position": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p]),
     "evo_decode_qkv_prep_rows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int64, C.c_void_p]),
     "evo_decode_attn_rows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int64, C.c_int, C.c_float, C.c_void_p, C.c_size_t, C.c_void_p]),
     "evo_advance_positions": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_void_p]),

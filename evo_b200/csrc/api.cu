@@ -101,7 +101,7 @@ int device_sm_count() {
 
 extern "C" {
 const char* evo_last_error(void) { return evo::g_err; }
-int evo_abi_version(void) { return 1; }
+int evo_abi_version(void) { return 2; }
 int64_t evo_launch_count(void) { return evo::g_launches.load(); }
 void evo_reset_launch_count(void) { evo::g_launches.store(0); }
 void evo_note_graph_replay(int64_t launches) { evo::g_launches.fetch_add(launches); }

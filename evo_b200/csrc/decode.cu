@@ -5,7 +5,6 @@
 #include "common.cuh"
 #include "wgmma.cuh"
 #include "../../include/evo_b200.h"
-#include <cstdlib>
 
 using namespace evo;
 
@@ -483,8 +482,6 @@ __global__ void decode_attn_merge2_kernel(const float* __restrict__ p_o, const f
   out[((long long)b * H + h) * HD + d] = __float2bfloat16_rn(acc / L);
 }
 
-__global__ void add_i64_kernel(long long* p, long long v) { *p += v; }
-
 __global__ void add_i64_rows_kernel(long long* p, int n, long long v) {
   pdl_launch_dependents(); pdl_wait();
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -526,9 +523,8 @@ extern "C" size_t evo_decode_attn_workspace(int B, int H, int nsplit) { return (
 // multiple of 64, the per-thread-row kernel otherwise
 static int decode_attn_partials(const char* what, const void* qkv, const void* cache, float* part_o, float* part_ml, const int64_t* pos, int pos_stride,
                                 int B, int H, int64_t max_seqlen, int nsplit, float softmax_scale, void* stream) {
-  static const bool force_v1 = getenv("EVO_B200_DECODE_ATTN_V1") != nullptr;
   int rc;
-  if (max_seqlen % TK == 0 && !force_v1 && (long long)B * max_seqlen < (1LL << 31)) {
+  if (max_seqlen % TK == 0 && (long long)B * max_seqlen < (1LL << 31)) {
     CUtensorMap tm;
     const uint64_t dims[3] = {(uint64_t)HD, (uint64_t)(2 * H), (uint64_t)B * (uint64_t)max_seqlen};
     const uint64_t str[2] = {(uint64_t)HD * 2, (uint64_t)2 * H * HD * 2};
@@ -567,11 +563,6 @@ extern "C" int evo_decode_attn(const void* qkv, const void* cache, void* out, co
 extern "C" int evo_decode_attn_rows(const void* qkv, const void* cache, void* out, const int64_t* pos, int B, int H, int hd,
                                     int64_t max_seqlen, int nsplit, float softmax_scale, void* workspace, size_t workspace_bytes, void* stream) {
   return decode_attn("evo_decode_attn_rows", qkv, cache, out, pos, 1, B, H, hd, max_seqlen, nsplit, softmax_scale, workspace, workspace_bytes, stream);
-}
-
-extern "C" int evo_advance_position(int64_t* pos, int64_t delta, void* stream) {
-  add_i64_kernel<<<1, 1, 0, (cudaStream_t)stream>>>((long long*)pos, delta);
-  return check_launch("evo_advance_position");
 }
 
 extern "C" int evo_advance_positions(int64_t* pos, int B, int64_t delta, void* stream) {

@@ -22,7 +22,6 @@
 #include "../../include/evo_b200.h"
 #include <algorithm>
 #include <cmath>
-#include <cstdlib>
 
 using namespace evo;
 
@@ -36,6 +35,7 @@ constexpr int NTHREADS = 384;
 constexpr int CONSUMER_WARPS = 8;
 constexpr int STG_LD = WROWS + 4;      // staging row stride (floats): conflict-free fragment stores
 constexpr int MAX_MB = 64;
+constexpr int RING_BYTES = 104 * 1024;  // shared memory for the W + A ring (152 KB measured the same, 208 KB slower)
 
 struct SmArgs {
   bf16* C; long long ldc;
@@ -44,11 +44,6 @@ struct SmArgs {
   int M, Mb;                        // rows of A; rows staged / UMMA N (multiple of 16)
   int n_tiles, KB;                  // tiles of (128*R) W rows; k-blocks per tile
   int n_stages;
-  // EPI_HYENA_STEP (fused engine.step_fir + step_iir behind the in-projection): the tile is one head's [x2 | x1 | v] rows
-  bf16* fir_state; float* state;    // (B, 3D, 2) bf16, (B, D, 8, 2) fp32: updated in place
-  const bf16* fir_w; const bf16* fir_b; const bf16* Dskip;
-  const float* poles; const float* residues;
-  int D;
   int* counters;                    // [n_tiles], zero between launches
   float* slots;                     // [2 * gridDim.x][R * Mb][128] fp32 partials
 };
@@ -95,71 +90,7 @@ __device__ __forceinline__ void finalize16(const SmArgs& g, long long n, int b0,
   }
 }
 
-constexpr int EPI_HYENA_STEP = 7;   // EVO_EPI_HYENA_STEP
-template <int EPI> struct RowGroups { static constexpr int R = EPI == EVO_EPI_GELU_GATE ? 2 : (EPI == EPI_HYENA_STEP ? 3 : 1); };
-
-// One decode step of the Hyena operator for channel `ch` of head `tile`, 16 batch rows: the arithmetic of hyena_step_kernel
-// (hyena.cu; engine.step_fir + step_iir of the reference) on the in-projection's fp32 sums z2/z1/zv (x2, x1, v rows of the head).
-// Every rounding point is the one the two-kernel path has: z = bf16(sum + bias), as EVO_EPI_BIAS stores it.  The fp32 sum itself
-// equals that launch's only where both cut the K range at the same k-blocks (the tile count, and so the stream-K split, differs).
-__device__ __forceinline__ void hyena_step16(const SmArgs& g, int tile, int row, int b0, const float (&z2)[16], const float (&z1)[16], const float (&zv)[16]) {
-  const int D = g.D, ch = tile * WROWS + row;
-  const long long C3 = 3LL * D;
-  const long long c_base = (long long)tile * 3 * WROWS + row;          // z column of x2; x1 = +128, v = +256
-  float w[3][3], fb[3], pb[3];
-#pragma unroll
-  for (int ci = 0; ci < 3; ++ci) {
-    const long long c = c_base + ci * WROWS;
-#pragma unroll
-    for (int k = 0; k < 3; ++k) w[ci][k] = __bfloat162float(g.fir_w[c * 3 + k]);
-    fb[ci] = __bfloat162float(g.fir_b[c]);
-    pb[ci] = __bfloat162float(g.bias[c]);
-  }
-  const float dskip = __bfloat162float(g.Dskip[ch]);
-  float2 p[8], r[8];
-#pragma unroll
-  for (int s = 0; s < 8; ++s) {
-    p[s] = reinterpret_cast<const float2*>(g.poles)[(long long)ch * 8 + s];
-    r[s] = reinterpret_cast<const float2*>(g.residues)[(long long)ch * 8 + s];
-  }
-#pragma unroll
-  for (int j = 0; j < 16; ++j) {
-    const int b = b0 + j;
-    if (b >= g.M) continue;
-    float f[3];
-    const float zin[3] = {z2[j], z1[j], zv[j]};
-#pragma unroll
-    for (int ci = 0; ci < 3; ++ci) {
-      const long long c = c_base + ci * WROWS;
-      const bf16 un_b = __float2bfloat16_rn(zin[ci] + pb[ci]);
-      const float un = __bfloat162float(un_b);
-      bf16* fs = g.fir_state + ((long long)b * C3 + c) * 2;
-      const bf16 s1_b = fs[1];
-      const float s0 = __bfloat162float(fs[0]), s1 = __bfloat162float(s1_b);
-      const float t0 = rbf(w[ci][2] * un);
-      const float t1 = rbf(rbf(s0 * w[ci][0]) + rbf(s1 * w[ci][1]));
-      f[ci] = rbf(rbf(t0 + t1) + fb[ci]);
-      fs[0] = s1_b; fs[1] = un_b;
-    }
-    const float x = rbf(f[1] * f[2]);
-    float4* st = reinterpret_cast<float4*>(g.state + ((long long)b * D + ch) * 16);
-    float4 sv[4];
-#pragma unroll
-    for (int q = 0; q < 4; ++q) sv[q] = st[q];
-    float acc = 0.f;
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      const float nr0 = fmaf(p[2 * q].x, sv[q].x, fmaf(-p[2 * q].y, sv[q].y, x));
-      const float ni0 = fmaf(p[2 * q].x, sv[q].y, p[2 * q].y * sv[q].x);
-      acc = fmaf(r[2 * q].x, nr0, acc); acc = fmaf(-r[2 * q].y, ni0, acc);
-      const float nr1 = fmaf(p[2 * q + 1].x, sv[q].z, fmaf(-p[2 * q + 1].y, sv[q].w, x));
-      const float ni1 = fmaf(p[2 * q + 1].x, sv[q].w, p[2 * q + 1].y * sv[q].z);
-      acc = fmaf(r[2 * q + 1].x, nr1, acc); acc = fmaf(-r[2 * q + 1].y, ni1, acc);
-      st[q] = make_float4(nr0, ni0, nr1, ni1);
-    }
-    g.C[(long long)b * g.ldc + ch] = __float2bfloat16_rn(f[0] * (acc + rbf(dskip * x)));
-  }
-}
+template <int EPI> struct RowGroups { static constexpr int R = EPI == EVO_EPI_GELU_GATE ? 2 : 1; };
 
 template <int MB>
 __device__ __forceinline__ void wgmma_ss_n(float (&d)[MB / 2], uint64_t da, uint64_t db, int scale_d) {
@@ -286,16 +217,14 @@ gemm_smallm_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constan
       if constexpr (EPI == EVO_EPI_BIAS || EPI == EVO_EPI_BIAS_RESID) bias = __bfloat162float(g.bias[n]);
       if (whole) {
         for (int c = cw * 16; c < MB; c += 32) {
-          float rv[16], v0[16], v1[16], v2[16];
+          float rv[16], v0[16], v1[16];
           load_resid16<EPI>(g, n, c, rv);
 #pragma unroll
           for (int j = 0; j < 16; ++j) {
             v0[j] = stg[(c + j) * STG_LD + row];
             v1[j] = R >= 2 ? stg[(MB + c + j) * STG_LD + row] : 0.f;
-            v2[j] = R == 3 ? stg[(2 * MB + c + j) * STG_LD + row] : 0.f;
           }
-          if constexpr (EPI == EPI_HYENA_STEP) hyena_step16(g, tile, row, c, v0, v1, v2);
-          else finalize16<EPI>(g, n, c, bias, rv, v0, v1);
+          finalize16<EPI>(g, n, c, bias, rv, v0, v1);
         }
       } else {
         float* slot = g.slots + (size_t)(2 * blockIdx.x + (tile == my_first_tile ? 0 : 1)) * slot_floats;
@@ -317,14 +246,14 @@ gemm_smallm_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constan
         const bool last = *flag == c_last - c_first;
         if (last) {
           for (int c = cw * 16; c < MB; c += 32) {
-            float v0[16], v1[16], v2[16], rv[16];
+            float v0[16], v1[16], rv[16];
             load_resid16<EPI>(g, n, c, rv);
 #pragma unroll
-            for (int j = 0; j < 16; ++j) { v0[j] = 0.f; v1[j] = 0.f; v2[j] = 0.f; }
+            for (int j = 0; j < 16; ++j) { v0[j] = 0.f; v1[j] = 0.f; }
             // slots are summed in contributor order (deterministic); the loads of FX contributors are in flight together
-            constexpr int FX = R == 3 ? 1 : (R == 2 ? 2 : 4);
+            constexpr int FX = R == 2 ? 2 : 4;
             for (int cb = c_first; cb <= c_last; cb += FX) {
-              float t0v[FX][16], t1v[FX][16], t2v[FX][16];
+              float t0v[FX][16], t1v[FX][16];
 #pragma unroll
               for (int u = 0; u < FX; ++u) {
                 const int cc = min(cb + u, c_last);
@@ -334,19 +263,17 @@ gemm_smallm_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constan
                 for (int j = 0; j < 16; ++j) {
                   t0v[u][j] = __ldcg(s + (c + j) * WROWS + row);
                   if constexpr (R >= 2) t1v[u][j] = __ldcg(s + (MB + c + j) * WROWS + row);
-                  if constexpr (R == 3) t2v[u][j] = __ldcg(s + (2 * MB + c + j) * WROWS + row);
                 }
               }
 #pragma unroll
               for (int u = 0; u < FX; ++u) {
                 if (cb + u <= c_last) {
 #pragma unroll
-                  for (int j = 0; j < 16; ++j) { v0[j] += t0v[u][j]; if constexpr (R >= 2) v1[j] += t1v[u][j]; if constexpr (R == 3) v2[j] += t2v[u][j]; }
+                  for (int j = 0; j < 16; ++j) { v0[j] += t0v[u][j]; if constexpr (R >= 2) v1[j] += t1v[u][j]; }
                 }
               }
             }
-            if constexpr (EPI == EPI_HYENA_STEP) hyena_step16(g, tile, row, c, v0, v1, v2);
-            else finalize16<EPI>(g, n, c, bias, rv, v0, v1);
+            finalize16<EPI>(g, n, c, bias, rv, v0, v1);
           }
           if (threadIdx.x == 128) g.counters[tile] = 0;      // self-cleaning for the next launch
         }
@@ -355,12 +282,6 @@ gemm_smallm_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constan
       it += k1 - k0;
     }
   }
-}
-
-int smem_budget_bytes() {
-  static int kb = 0;
-  if (!kb) { const char* e = getenv("EVO_B200_SMALLM_SMEM_KB"); kb = e ? atoi(e) : 104; kb = std::max(40, std::min(kb, 224)); }
-  return kb * 1024;
 }
 
 template <int EPI, int MB>
@@ -373,14 +294,11 @@ int launch(const evo_gemm_smallm_params* p, cudaStream_t st) {
   SmArgs g;
   g.C = (bf16*)p->C; g.ldc = p->ldc; g.bias = (const bf16*)p->bias; g.resid = (const bf16*)p->residual; g.ldr = p->ldr;
   g.M = (int)p->M; g.Mb = MB;
-  g.fir_state = (bf16*)p->fir_state; g.state = p->state; g.fir_w = (const bf16*)p->fir_w; g.fir_b = (const bf16*)p->fir_b; g.Dskip = (const bf16*)p->Dskip;
-  g.poles = p->poles; g.residues = p->residues; g.D = (int)(p->N / 3);
   g.n_tiles = (int)(p->N / (R * WROWS));
   g.KB = (int)(p->K / BK);
   const int stage_bytes = R * WROWS * BK * 2 + MB * BK * 2;
   const int tail = R * MB * STG_LD * 4 + 2 * MAXST * 8 + 16;
-  // three row groups stage 48 KB of W per k-block: give the ring 160 KB (3 stages) instead of the default budget (2)
-  const int budget = std::min(R == 3 ? std::max(smem_budget_bytes(), 160 * 1024) : smem_budget_bytes(), 227 * 1024 - tail);
+  const int budget = std::min(RING_BYTES, 227 * 1024 - tail);
   g.n_stages = std::max(2, std::min(MAXST, budget / stage_bytes));
   const int smem_bytes = g.n_stages * stage_bytes + tail;
   const long long total = (long long)g.n_tiles * g.KB;
@@ -423,7 +341,7 @@ int launch_mb(const evo_gemm_smallm_params* p, cudaStream_t st) {
 
 extern "C" size_t evo_gemm_smallm_workspace(int64_t M, int64_t N, int64_t K, int epilogue) {
   (void)K;
-  const int R = epilogue == EVO_EPI_GELU_GATE ? 2 : (epilogue == EPI_HYENA_STEP ? 3 : 1);
+  const int R = epilogue == EVO_EPI_GELU_GATE ? 2 : 1;
   const size_t Mb = (size_t)((M + 15) / 16 * 16);
   if (N / (R * WROWS) > 4096) return 0;
   return 16384 + (size_t)2 * device_sm_count() * R * Mb * WROWS * sizeof(float);
@@ -435,7 +353,6 @@ extern "C" int evo_gemm_smallm(const evo_gemm_smallm_params* p, void* stream) {
   EVO_REQUIRE(p->N % 256 == 0 && p->N / WROWS <= 4096, "evo_gemm_smallm: N (%lld) must be a multiple of 256 (and <= 524288)", (long long)p->N);
   EVO_REQUIRE(p->lda % 8 == 0, "evo_gemm_smallm: lda must be a multiple of 8 elements");
   EVO_REQUIRE(((uintptr_t)p->A % 16) == 0 && ((uintptr_t)p->W % 16) == 0, "evo_gemm_smallm: A and W must be 16-byte aligned");
-  static_assert(EPI_HYENA_STEP == EVO_EPI_HYENA_STEP, "enum drift");
   if (p->epilogue == EVO_EPI_BIAS || p->epilogue == EVO_EPI_BIAS_RESID) EVO_REQUIRE(p->bias != nullptr, "evo_gemm_smallm: bias epilogue without bias");
   if (p->epilogue == EVO_EPI_RESID || p->epilogue == EVO_EPI_BIAS_RESID) EVO_REQUIRE(p->residual != nullptr, "evo_gemm_smallm: residual epilogue without residual");
   if (p->M == 0) return 0;
@@ -445,10 +362,6 @@ extern "C" int evo_gemm_smallm(const evo_gemm_smallm_params* p, void* stream) {
     case EVO_EPI_BIAS_RESID: return launch_mb<EVO_EPI_BIAS_RESID>(p, (cudaStream_t)stream);
     case EVO_EPI_RESID: return launch_mb<EVO_EPI_RESID>(p, (cudaStream_t)stream);
     case EVO_EPI_GELU_GATE: return launch_mb<EVO_EPI_GELU_GATE>(p, (cudaStream_t)stream);
-    case EPI_HYENA_STEP:
-      EVO_REQUIRE(p->bias && p->fir_state && p->state && p->fir_w && p->fir_b && p->Dskip && p->poles && p->residues, "evo_gemm_smallm: EVO_EPI_HYENA_STEP needs bias, states and filter parameters");
-      EVO_REQUIRE(p->N % (3 * WROWS) == 0, "evo_gemm_smallm: EVO_EPI_HYENA_STEP needs N = 3 * heads * 128");
-      return launch_mb<EPI_HYENA_STEP>(p, (cudaStream_t)stream);
   }
   set_error("evo_gemm_smallm: unknown epilogue %d", p->epilogue);
   return -1;

@@ -553,6 +553,7 @@ int dispatch_epi(const evo_gemm_params* p, cudaStream_t st) {
 
 extern "C" int evo_gemm(const evo_gemm_params* p, void* stream) {
   EVO_REQUIRE(p->M >= 0 && p->N > 0 && p->K > 0, "evo_gemm: bad shape");
+  EVO_REQUIRE(p->variant >= 0 && p->variant <= 3, "evo_gemm: unknown variant %d", p->variant);
   EVO_REQUIRE(p->K % BK == 0, "evo_gemm: K (%lld) must be a multiple of %d", (long long)p->K, BK);
   EVO_REQUIRE(p->N % BN_BIG == 0, "evo_gemm: N (%lld) must be a multiple of %d (pack weights at load time)", (long long)p->N, BN_BIG);
   EVO_REQUIRE(p->lda % 8 == 0 && p->ldc % 8 == 0, "evo_gemm: lda/ldc must be multiples of 8 elements");

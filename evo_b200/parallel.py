@@ -27,6 +27,7 @@ import torch.distributed as dist
 
 from . import _lib
 from ._lib import EPI_BIAS, EPI_BIAS_RESID, EPI_BIAS_ROPE, AttnParams, HyenaParams, check, ptr
+from .stripedhyena.model import ATTN_VARIANT
 
 
 # attention re-shard through our own NVLink peer stores (PeerUlysses) instead of NCCL all-to-alls; "0" = NCCL Ulysses.
@@ -147,7 +148,7 @@ def _peer_attention(model, lib, pu, xn, mha, u, B, Lr, H, hd, rank, world, strea
     ap.k, ap.v, ap.kv_tok_stride, ap.kv_batch_stride = full.data_ptr() + dl * 2, full.data_ptr() + 2 * dl * 2, 3 * dl, L * 3 * dl
     ap.out_peers, ap.n_out_peers, ap.out_rows_per_peer, ap.out_row_stride, ap.out_col0 = C.cast(pu.ctx_ptrs, C.c_void_p), world, Lr, d, rank * dl
     causal_flops = 4.0 * pu.Hl * hd * (L * (L + 1) / 2.0)
-    model._record("attn", causal_flops, lambda: check(lib.evo_attn_fwd_ws(C.byref(ap), model.attn_variant, None, 0, stream()), "evo_attn_fwd(peer)"))
+    model._record("attn", causal_flops, lambda: check(lib.evo_attn_fwd_ws(C.byref(ap), ATTN_VARIANT, None, 0, stream()), "evo_attn_fwd(peer)"))
     pu.signal_and_wait(model, lib, "c", stream)
     return pu.ctx()
 
@@ -176,7 +177,7 @@ def _ulysses_attention(model, lib, qkv, ctx, B, Lr, H, hd, rank, world, group, s
     ap.q, ap.q_tok_stride, ap.q_batch_stride = full.data_ptr(), 3 * dl, L * 3 * dl
     ap.k, ap.v, ap.kv_tok_stride, ap.kv_batch_stride = full.data_ptr() + dl * 2, full.data_ptr() + 2 * dl * 2, 3 * dl, L * 3 * dl
     causal_flops = 4.0 * B * Hl * hd * (L * (L + 1) / 2.0)
-    model._launch_ws("attn", causal_flops, "evo_attn_fwd", lib.evo_attn_fwd_workspace, lib.evo_attn_fwd_ws, ap, model.attn_variant)
+    model._launch_ws("attn", causal_flops, "evo_attn_fwd", lib.evo_attn_fwd_workspace, lib.evo_attn_fwd_ws, ap, ATTN_VARIANT)
     # back: (B, P, Lr, Hl*hd) -> chunk p (its tokens, my heads) to rank p
     if B == 1:
         send2 = out.view(world, B, Lr, dl)            # chunk p = tokens of rank p: already contiguous
@@ -216,7 +217,7 @@ def sequence_parallel_forward(model, ids_local: torch.Tensor, rank: int, world: 
             # hang, so every rank learns whether ALL of them have the peer path
             pu = None
             rope_fused = all(model._rope_fused(model.blocks[j].inner_mha_cls) for j in model._attn_idxs)    # the peer scatter is that epilogue's
-            if PEER_ULYSSES and pc is not None and B == 1 and H % world == 0 and hd == 128 and rope_fused and model.attn_variant in (2, 3):
+            if PEER_ULYSSES and pc is not None and B == 1 and H % world == 0 and hd == 128 and rope_fused:
                 try:
                     pu = PeerUlysses(world, rank, Lr, d, H, dev, group)
                 except Exception as ex:  # noqa

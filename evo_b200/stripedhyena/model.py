@@ -26,14 +26,12 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from .. import _lib
-from .._lib import (EPI_BIAS, EPI_BIAS_RESID, EPI_BIAS_ROPE, EPI_GELU_GATE, EPI_HYENA_STEP, EPI_NONE, EPI_RESID, AttnParams, AttnVarlenParams,
+from .._lib import (EPI_BIAS, EPI_BIAS_RESID, EPI_BIAS_ROPE, EPI_GELU_GATE, EPI_NONE, EPI_RESID, AttnParams, AttnVarlenParams,
                     AttnVarlenPrefixParams, GemmParams, GemmSmallMParams, HyenaParams, HyenaVarlenCkptParams, HyenaVarlenParams, check, ptr)
 from .cache import InferenceParams, RecurrentInferenceParams
 
-# kernel variants (see include/evo_b200.h); overridable for experiments
-GEMM_VARIANT = int(os.environ.get("EVO_B200_GEMM_VARIANT", "0"))
-GEMM_VARIANT_GATE = int(os.environ.get("EVO_B200_GEMM_VARIANT_GATE", "0"))
-ATTN_VARIANT = int(os.environ.get("EVO_B200_ATTN_VARIANT", "2"))
+# attention variant passed to evo_attn_fwd_ws: every variant runs the same kernel, and 2 also accepts peer-scattered output
+ATTN_VARIANT = 2
 
 
 def _round_up(x: int, m: int) -> int:
@@ -305,24 +303,13 @@ class StripedHyena(nn.Module):
         self._attn_idxs = attn
         self._packed = None
         self._rope = None
-        self.gemm_variant = GEMM_VARIANT
-        self.gemm_variant_gate = GEMM_VARIANT_GATE
-        self.attn_variant = ATTN_VARIANT
         self.decode_graph = os.environ.get("EVO_B200_DECODE_GRAPH", "1") != "0"
-        # rotary embedding inside the Wqkv GEMM's epilogue (EVO_EPI_BIAS_ROPE) instead of a separate pass over qkv; "0" = separate evo_rotary_qk
-        self.fused_rope = os.environ.get("EVO_B200_FUSED_ROPE", "1") != "0"
         # tile-major weight copies for decode (GEMM variant 3): bit-identical to variant 2; off unless measured faster
         self.decode_tiled = os.environ.get("EVO_B200_DECODE_TILED", "0") != "0"
         # decode-step GEMMs: stream-K weight-streaming kernel (csrc/gemm_smallm.cu) for batch <= 64; "0" = the 128x64 tiles
         self.decode_streamk = os.environ.get("EVO_B200_DECODE_STREAMK", "1") != "0"
         # programmatic dependent launch inside a decode step (evo_set_pdl): 0 off, 1 every kernel, 2 weight-streaming GEMMs only
         self.decode_pdl = int(os.environ.get("EVO_B200_DECODE_PDL", "4"))
-        # the Hyena decode step inside the in-projection GEMM's epilogue (EVO_EPI_HYENA_STEP).  The step arithmetic is bit-identical
-        # to the separate evo_hyena_step launch; z matches EVO_EPI_BIAS up to the stream-K split of the K sum, which depends on the tile
-        # height (DESIGN.md).  The step of a tile runs on the 128 epilogue threads of its last contributor -- 16 batch rows x 8 states of dependent
-        # load -> update -> store per thread in the GEMM's serial tail -- where the stand-alone kernel spreads the same 8 MB of state
-        # traffic over 524 288 threads.  Off by default; kept as a tested option.
-        self.decode_fused_step = os.environ.get("EVO_B200_DECODE_FUSED_STEP", "0") != "0"
         self._smallm_ws = None
         self._tiled = None   # tile-major weight copies for the weight-streaming decode GEMMs
         self._decode = None  # cached CUDA graph of one decode step (see _decode_forward)
@@ -407,11 +394,9 @@ class StripedHyena(nn.Module):
         e1.record()
         self._prof.append((kind, work, e0, e1))
 
-    def _gemm(self, a, w, out, M, N, K, epi, bias=None, resid=None, ldc=None, variant=None, rope=None, peers=None):
+    def _gemm(self, a, w, out, M, N, K, epi, bias=None, resid=None, ldc=None, variant=0, rope=None, peers=None):
         """rope = (cos_ptr, sin_ptr, tokens_per_sequence, rotated_columns) for EPI_BIAS_ROPE;
         peers = (ctypes array of peer pointers, n, period, inner, row0): peer-scattered output (see evo_gemm_params), out may be None."""
-        if variant is None:
-            variant = self.gemm_variant_gate if epi == EPI_GELU_GATE else self.gemm_variant
         p = GemmParams(A=a.data_ptr(), lda=K, W=w.data_ptr(), C=out.data_ptr() if out is not None else None, ldc=ldc or N,
                        bias=bias.data_ptr() if bias is not None else None,
                        residual=resid.data_ptr() if resid is not None else None, ldr=ldc or N,
@@ -423,27 +408,20 @@ class StripedHyena(nn.Module):
             p.c_peers, p.n_c_peers, p.peer_period, p.peer_inner, p.peer_row0 = C.cast(arr, C.c_void_p), n, period, inner, row0
         self._record(f"gemm/{N}x{K}/e{epi}/v{variant}", 2.0 * M * N * K, lambda: check(_lib.lib().evo_gemm(C.byref(p), self._stream()), "evo_gemm"))
 
-    def _gemm_smallm(self, a, w, out, M, N, K, epi, bias=None, resid=None, step=None):
-        """Decode-step linear layer (M <= 64): stream-K weight-streaming kernel, gate epilogue fused.
-        step = (fir_state, state_real, filter module) for EPI_HYENA_STEP: the in-projection with the operator's decode step
-        in its epilogue (out is then y (M, N/3))."""
+    def _gemm_smallm(self, a, w, out, M, N, K, epi, bias=None, resid=None):
+        """Decode-step linear layer (M <= 64): stream-K weight-streaming kernel, gate epilogue fused."""
         lib = _lib.lib()
         need = lib.evo_gemm_smallm_workspace(M, N, K, epi)
         ws = self._smallm_ws
         if ws is None or ws.numel() < need or ws.device != a.device:
             self._decode = None      # a captured decode graph holds the old workspace address
-            ws = self._smallm_ws = torch.zeros(max(need, lib.evo_gemm_smallm_workspace(M, 256, 64, EPI_GELU_GATE), lib.evo_gemm_smallm_workspace(M, 384, 64, EPI_HYENA_STEP)),
+            ws = self._smallm_ws = torch.zeros(max(need, lib.evo_gemm_smallm_workspace(M, 256, 64, EPI_GELU_GATE)),
                                                dtype=torch.uint8, device=a.device)
-        n_out = N // 2 if epi == EPI_GELU_GATE else (N // 3 if epi == EPI_HYENA_STEP else N)
+        n_out = N // 2 if epi == EPI_GELU_GATE else N
         p = GemmSmallMParams(A=a.data_ptr(), lda=K, W=w.data_ptr(), C=out.data_ptr(), ldc=n_out,
                              bias=bias.data_ptr() if bias is not None else None,
                              residual=resid.data_ptr() if resid is not None else None, ldr=n_out,
                              M=M, N=N, K=K, epilogue=epi, workspace=ws.data_ptr(), workspace_bytes=ws.numel())
-        if step is not None:
-            fs, st, f = step
-            p.fir_state, p.state = fs.data_ptr(), st.data_ptr()
-            for name, v in f.ptrs().items():
-                setattr(p, name, v)
         self._record(f"gemm/{N}x{K}/e{epi}/streamk", 2.0 * M * N * K, lambda: check(lib.evo_gemm_smallm(C.byref(p), self._stream()), "evo_gemm_smallm"))
 
     def _rmsnorm(self, x, scale, out, rows):
@@ -567,10 +545,10 @@ class StripedHyena(nn.Module):
         return cos.data_ptr() + off, sin.data_ptr() + off
 
     def _rope_fused(self, mha):
-        """Whether the Wqkv GEMM applies rotary in its epilogue (EVO_EPI_BIAS_ROPE: bias + rotary, head_dim 128, GEMM variants
-        0 and 1), where flash_attn's MHA applies it (mha.py:635-648); otherwise a second pass over qkv does."""
+        """Whether the Wqkv GEMM applies rotary in its epilogue (EVO_EPI_BIAS_ROPE: bias + rotary, head_dim 128), where
+        flash_attn's MHA applies it (mha.py:635-648); otherwise a second pass over qkv does."""
         hd = self.config.hidden_size // self.config.num_attention_heads
-        return self.fused_rope and mha.Wqkv.bias is not None and hd == 128 and self.gemm_variant in (0, 1)
+        return mha.Wqkv.bias is not None and hd == 128
 
     def _qkv_rope(self, xn, mha, qkv, B, L, rope):
         """qkv (B*L, 3D) = Wqkv xn (+ bias), rotary on q and k from rope = (cos, sin) addresses of each sequence's L rows."""
@@ -633,7 +611,7 @@ class StripedHyena(nn.Module):
                 ap.k, ap.v = cache.data_ptr(), cache.data_ptr() + d * 2
                 ap.kv_tok_stride, ap.kv_batch_stride, ap.Lk = 2 * d, cache.shape[1] * 2 * d, off + L
             causal_flops = 4.0 * B * H * hd * (L * (off + (L + 1) / 2.0))   # QK^T + PV over the visible (query, key) pairs
-            self._launch_ws("attn", causal_flops, "evo_attn_fwd", lib.evo_attn_fwd_workspace, lib.evo_attn_fwd_ws, ap, self.attn_variant)
+            self._launch_ws("attn", causal_flops, "evo_attn_fwd", lib.evo_attn_fwd_workspace, lib.evo_attn_fwd_ws, ap, ATTN_VARIANT)
         return self._mlp_residual(i, blk, self._out_proj(mha, ctx, u), M)
 
     def _attention_varlen(self, i, qkv, ctx, vl, ip):
@@ -1006,18 +984,11 @@ class StripedHyena(nn.Module):
                 lin(ctx, wsel(i, "out", mha.out_proj.weight), u2, d, d, EPI_BIAS_RESID if mha.out_proj.bias is not None else EPI_RESID,
                     bias=mha.out_proj.bias, resid=u)
             else:
-                f = blk.filter
-                if streamk and self.decode_fused_step and hd == 128:
-                    # in-projection with engine.step_fir + step_iir in its epilogue: z never leaves the SM, one launch less per layer
-                    y = torch.empty(B, d, dtype=torch.bfloat16, device=dev)
-                    self._gemm_smallm(xn, blk.projections.weight, y, B, 3 * d, d, EPI_HYENA_STEP, bias=blk.projections.bias,
-                                      step=(hy_ip.fir_state_dict[i], torch.view_as_real(hy_ip.state_dict[i]), f))
-                else:
-                    z = torch.empty(B, 3 * d, dtype=torch.bfloat16, device=dev)
-                    lin(xn, wsel(i, "in", blk.projections.weight), z, 3 * d, d, EPI_BIAS, bias=blk.projections.bias)
-                    y = xn
-                    check(lib.evo_hyena_step(ptr(z), ptr(y), ptr(hy_ip.fir_state_dict[i]), ptr(torch.view_as_real(hy_ip.state_dict[i])),
-                                             *map(C.c_void_p, f.ptrs().values()), B, d, cfg.state_size, H, self._stream()), "evo_hyena_step")
+                z = torch.empty(B, 3 * d, dtype=torch.bfloat16, device=dev)
+                lin(xn, wsel(i, "in", blk.projections.weight), z, 3 * d, d, EPI_BIAS, bias=blk.projections.bias)
+                y = xn
+                check(lib.evo_hyena_step(ptr(z), ptr(y), ptr(hy_ip.fir_state_dict[i]), ptr(torch.view_as_real(hy_ip.state_dict[i])),
+                                         *map(C.c_void_p, blk.filter.ptrs().values()), B, d, cfg.state_size, H, self._stream()), "evo_hyena_step")
                 lin(y, wsel(i, "out", blk.out_filter_dense.weight), u2, d, d, EPI_BIAS_RESID, bias=blk.out_filter_dense.bias, resid=u)
             pk = self._packed[i]
             xn2 = xn

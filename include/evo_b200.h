@@ -56,9 +56,6 @@ enum {
   EVO_EPI_RESID = 3,      /* C = bf16(bf16(acc) + R[m,n])           l3(...) + u           */
   EVO_EPI_GELU_GATE = 4,  /* W rows interleaved in 128-row groups [l1 | l2]; C[M,N/2] =
                              bf16(gelu(bf16(acc1)) * bf16(acc2))    act(l1 x) * l2 x      */
-  EVO_EPI_HYENA_STEP = 7, /* evo_gemm_smallm only: the Hyena in-projection (N = 3D, bias) with the decode step of the operator
-                             (engine.step_fir + step_iir == evo_hyena_step) applied in the epilogue: a tile is one head's
-                             [x2 | x1 | v] rows, C is y (M, D); fir_state / state are updated in place; z is never stored */
   EVO_EPI_BIAS_ROPE = 6   /* Wqkv projection with the rotary embedding applied where flash_attn applies it
                              (MHA.forward, mha.py:635-648): x = bf16(acc + bias[n]); columns n < rope_cols (q and k,
                              heads of 128) are rotated NeoX-style with the cos/sin row of the token's position
@@ -74,7 +71,8 @@ typedef struct {
   int64_t M, N, K;
   int epilogue;
   int variant;                   /* 0, 1 = 128x256 tiles; 2 = 128x64 weight-streaming tiles (small M);
-                                    3 = like 2 with W given tile-major: (N/64, K/64, 64, 64), i.e. W.view(N/64,64,K/64,64).permute(0,2,1,3) */
+                                    3 = like 2 with W given tile-major: (N/64, K/64, 64, 64), i.e. W.view(N/64,64,K/64,64).permute(0,2,1,3);
+                                    any other value is rejected */
   const void* rope_cos; const void* rope_sin;   /* EVO_EPI_BIAS_ROPE: (positions, 64) bf16 tables (evo_rope_tables) */
   int64_t rope_L;                /* tokens per sequence: row m uses table row m % rope_L */
   int64_t rope_cols;             /* columns [0, rope_cols) are rotated (2*H*128 for a qkv projection), the rest only get the bias */
@@ -102,10 +100,6 @@ typedef struct {
   int64_t M, N, K;               /* M <= 64, N % 256 == 0, K % 64 == 0 */
   int epilogue;                  /* EVO_EPI_* */
   void* workspace; size_t workspace_bytes;
-  /* EVO_EPI_HYENA_STEP only (same tensors as evo_hyena_step): */
-  void* fir_state; float* state;                 /* (M, 3D, 2) bf16, (M, D, 8, 2) fp32: in/out */
-  const void* fir_w; const void* fir_b; const void* Dskip;
-  const float* poles; const float* residues;
 } evo_gemm_smallm_params;
 size_t evo_gemm_smallm_workspace(int64_t M, int64_t N, int64_t K, int epilogue);
 int evo_gemm_smallm(const evo_gemm_smallm_params* p, void* stream);
@@ -277,7 +271,6 @@ int evo_kv_append_varlen(const void* qkv, void* cache, const int64_t* cu_seqlens
  * evo_decode_qkv_prep: rotary on q,k of qkv (B, 3, H, 128) at position *pos and append of k,v at cache row *pos
  *   (flash_attn_with_kvcache's rotary + cache-append half, mha.py:502-540).
  * evo_decode_attn: one query per sequence over cache keys [0, *pos] (the attention half); split-K over nsplit.
- * evo_advance_position: *pos += delta on the stream.
  * Per-row positions (a batch of prompts of different lengths): the _rows forms take pos as a (B) int64 DEVICE array and
  *   use pos[b] for row b -- rotary at pos[b], k,v appended at cache row pos[b], row b attends keys [0, pos[b]].  With every
  *   pos[b] equal they give the scalar forms' bits.  evo_advance_positions: pos[b] += delta for b < B. */
@@ -287,7 +280,6 @@ int evo_decode_qkv_prep(void* qkv, void* cache, const void* cos, const void* sin
 size_t evo_decode_attn_workspace(int B, int H, int nsplit);
 int evo_decode_attn(const void* qkv, const void* cache, void* out, const int64_t* pos, int B, int H, int hd,
                     int64_t max_seqlen, int nsplit, float softmax_scale, void* workspace, size_t workspace_bytes, void* stream);
-int evo_advance_position(int64_t* pos, int64_t delta, void* stream);
 int evo_decode_qkv_prep_rows(void* qkv, void* cache, const void* cos, const void* sin, const int64_t* pos,
                              int B, int H, int hd, int64_t max_seqlen, void* stream);
 int evo_decode_attn_rows(const void* qkv, const void* cache, void* out, const int64_t* pos, int B, int H, int hd,

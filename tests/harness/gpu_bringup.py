@@ -303,30 +303,28 @@ def stage_attn(variant):
 
 def stage_model():
     dev = "cuda:0"
-    for gv, av in ((0, 0), (1, 0), (0, 1)):
-        cfg = O.tiny_config(num_layers=4, attn_layer_idxs=(1, 3), hidden_size=256, num_heads=2)
-        sd = O.random_state_dict(cfg, seed=7)
-        m = StripedHyena(dotdict(cfg)); m.load_state_dict(sd, strict=True); m.to_bfloat16_except_poles_residues(); m = m.to(dev)
-        m.gemm_variant, m.gemm_variant_gate, m.attn_variant = gv, gv, av
-        ob = O.OracleStripedHyena(cfg, sd, torch.bfloat16); ot = O.OracleStripedHyena(cfg, sd, torch.float64)
-        torch.manual_seed(0)
-        ids = torch.randint(0, 4, (2, 333)) * 3 + 65
-        lg, _ = m(ids.to(dev)); torch.cuda.synchronize()
-        lb, _ = ob(ids); lt, _ = ot(ids)
-        lsm = lambda x: torch.log_softmax(x.double().cpu(), -1)
-        emit("model", gemm_variant=gv, attn_variant=av, logits_vs_oracle=err(lg, lb), logits_vs_truth=err(lg, lt), oracle_vs_truth=err(lb, lt),
-             logprob_mean_abs_vs_truth=(lsm(lg) - lsm(lt)).abs().mean().item(), oracle_logprob_mean_abs_vs_truth=(lsm(lb) - lsm(lt)).abs().mean().item(),
-             argmax_agree=(lg.cpu().argmax(-1) == lt.argmax(-1)).float().mean().item())
-        # stateful: prefill 300 then 33 steps, against the stateless logits
-        d = m.initialize_inference_params(); d["mha"].max_batch_size = 2; d["mha"].max_seqlen = 512
-        pre, d = m(ids[:, :300].to(dev), inference_params_dict=d)
-        errs = [err(pre, lg[:, :300])["max_abs"]]
-        d["mha"].seqlen_offset = d["hyena"].seqlen_offset = 300
-        for t in range(300, 333):
-            s, d = m(ids[:, t:t + 1].to(dev), inference_params_dict=d)
-            errs.append((s[:, 0].float() - lg[:, t].float()).abs().max().item())
-            d["mha"].seqlen_offset += 1; d["hyena"].seqlen_offset += 1
-        emit("model", gemm_variant=gv, attn_variant=av, stateful_prefill_max=errs[0], stateful_step_max=max(errs[1:]), logit_scale=lg.float().abs().max().item())
+    cfg = O.tiny_config(num_layers=4, attn_layer_idxs=(1, 3), hidden_size=256, num_heads=2)
+    sd = O.random_state_dict(cfg, seed=7)
+    m = StripedHyena(dotdict(cfg)); m.load_state_dict(sd, strict=True); m.to_bfloat16_except_poles_residues(); m = m.to(dev)
+    ob = O.OracleStripedHyena(cfg, sd, torch.bfloat16); ot = O.OracleStripedHyena(cfg, sd, torch.float64)
+    torch.manual_seed(0)
+    ids = torch.randint(0, 4, (2, 333)) * 3 + 65
+    lg, _ = m(ids.to(dev)); torch.cuda.synchronize()
+    lb, _ = ob(ids); lt, _ = ot(ids)
+    lsm = lambda x: torch.log_softmax(x.double().cpu(), -1)
+    emit("model", logits_vs_oracle=err(lg, lb), logits_vs_truth=err(lg, lt), oracle_vs_truth=err(lb, lt),
+         logprob_mean_abs_vs_truth=(lsm(lg) - lsm(lt)).abs().mean().item(), oracle_logprob_mean_abs_vs_truth=(lsm(lb) - lsm(lt)).abs().mean().item(),
+         argmax_agree=(lg.cpu().argmax(-1) == lt.argmax(-1)).float().mean().item())
+    # stateful: prefill 300 then 33 steps, against the stateless logits
+    d = m.initialize_inference_params(); d["mha"].max_batch_size = 2; d["mha"].max_seqlen = 512
+    pre, d = m(ids[:, :300].to(dev), inference_params_dict=d)
+    errs = [err(pre, lg[:, :300])["max_abs"]]
+    d["mha"].seqlen_offset = d["hyena"].seqlen_offset = 300
+    for t in range(300, 333):
+        s, d = m(ids[:, t:t + 1].to(dev), inference_params_dict=d)
+        errs.append((s[:, 0].float() - lg[:, t].float()).abs().max().item())
+        d["mha"].seqlen_offset += 1; d["hyena"].seqlen_offset += 1
+    emit("model", stateful_prefill_max=errs[0], stateful_step_max=max(errs[1:]), logit_scale=lg.float().abs().max().item())
 
 
 def stage_perf_gemm():
@@ -427,7 +425,7 @@ def stage_perf_decode():
     emit("perf_decode", B=B, prompt=P, steps=N, prefill_s=t_prefill, prefill_nt_s=B * P / t_prefill, first_step_ms=times[0] * 1e3, capture_step_ms=times[1] * 1e3,
          steady_ms_per_step=steady * 1e3, decode_nt_s=B / steady, decode_vs_stateless_max=e.max().item(), logit_scale=full.float().abs().max().item(),
          weight_stream_floor_ms=12.9e9 / 6566.4e9 * 1e3, eager_breakdown=breakdown,
-         env={k: os.environ.get(k) for k in ("EVO_B200_DECODE_STREAMK", "EVO_B200_DECODE_PDL", "EVO_B200_SMALLM_SMEM_KB", "EVO_B200_DECODE_GRAPH")})
+         env={k: os.environ.get(k) for k in ("EVO_B200_DECODE_STREAMK", "EVO_B200_DECODE_PDL", "EVO_B200_DECODE_GRAPH")})
 
 
 if __name__ == "__main__":

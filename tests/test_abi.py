@@ -35,9 +35,9 @@ def test_binding_table_covers_the_header():
     assert sorted(_lib.SIGNATURES) == header_functions()
 
 
-def test_loader_binds_and_reports_version():
+def test_loader_binds_and_reports_abi_version_2():
     lib = _lib.lib()
-    assert lib.evo_abi_version() == 1
+    assert lib.evo_abi_version() == 2
     assert lib.evo_last_error() is not None
     lib.evo_reset_launch_count()
     assert lib.evo_launch_count() == 0
@@ -62,7 +62,7 @@ def test_sass_has_wgmma_and_tma():
     assert "HMMA.16816" not in sass     # no legacy mma.sync tensor path
 
 
-def test_header_is_plain_c_and_a_c_host_binds_every_entry_point(tmp_path):
+def test_header_is_plain_c_and_a_c_host_binds_abi_version_2(tmp_path):
     """include/evo_b200.h is the boundary for ANY host: it must compile as C99 and as C++ on its own, and a C program that
     #includes it and dlopen()s the library must resolve every declared entry point and get answers from the two that need no
     GPU (no torch, no Python anywhere near this binding)."""
@@ -94,7 +94,7 @@ def test_header_is_plain_c_and_a_c_host_binds_every_entry_point(tmp_path):
     r = subprocess.run([gcc, "-std=gnu99", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe), "-ldl"], capture_output=True, text=True)
     assert r.returncode == 0, r.stderr
     r = subprocess.run([str(exe), _lib.LIB_PATH], capture_output=True, text=True)
-    assert r.returncode == 0 and r.stdout.split() == ["0", "1", "str"], (r.stdout, r.stderr)
+    assert r.returncode == 0 and r.stdout.split() == ["0", "2", "str"], (r.stdout, r.stderr)
 
 
 def test_error_convention_without_a_gpu():
@@ -107,6 +107,10 @@ def test_error_convention_without_a_gpu():
     lib = _lib.lib()
     p = _lib.GemmParams(A=0x1000, lda=100, W=0x2000, C=0x3000, ldc=64, bias=None, residual=None, ldr=64, M=4, N=64, K=100, epilogue=0, variant=0)
     assert lib.evo_gemm(ctypes.byref(p), None) < 0 and b"K (100) must be a multiple of 64" in lib.evo_last_error()
+    p.K, p.N, p.variant = 128, 256, 4
+    assert lib.evo_gemm(ctypes.byref(p), None) < 0 and b"evo_gemm: unknown variant 4" in lib.evo_last_error()
+    s = _lib.GemmSmallMParams(A=0x1000, lda=64, W=0x2000, C=0x3000, ldc=256, M=4, N=256, K=64, epilogue=7)
+    assert lib.evo_gemm_smallm(ctypes.byref(s), None) < 0 and b"evo_gemm_smallm: unknown epilogue 7" in lib.evo_last_error()
     assert lib.evo_sample(None, None, 2, 2000, 1, 0.0, 1.0, 0, 0, None) < 0 and b"vocabulary 2000 unsupported" in lib.evo_last_error()
     assert lib.evo_kv_append(None, None, 1, 10, 2, 128, 10, 16, None) < 0 and b"exceeds the KV cache (16)" in lib.evo_last_error()   # mha.py:367
     with pytest.raises(_lib.EvoError, match="exceeds the KV cache"):

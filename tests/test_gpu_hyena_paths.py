@@ -5,8 +5,8 @@ D % 256 == 0, and the scalar kernel (hyena_scan_kernel in hyena.cu) for every ot
 reference's bf16 rounding points, so both are held to the bars of
 tests/test_gpu_parity.py::test_hyena_operator_vs_oracle.  On top of the plain prefill this file covers the history
 inputs (halo, state_in), the carry passes the sequence-parallel forward chains (state_only with its fold kernel,
-evo_hyena_combine_states, reuse_segment_states), the decode step at the 7B width and at head_dim != 128, the decode step
-fused into the in-projection's epilogue, and the calls the launcher must reject.
+evo_hyena_combine_states, reuse_segment_states), the decode step at the 7B width and at head_dim != 128, and the calls
+the launcher must reject.
 
 References: the oracle's bf16 FFT operator (the reference's rounding points) and the fp64 time-domain recurrence
 O.hyena_operator_time_domain (the truth; it takes a halo and a modal state).  Where the FFT operator cannot express an
@@ -415,62 +415,6 @@ def test_decode_step_vs_oracle(D, H, B):
     e_ref = (ost - stb_f).abs().max().item() / scale
     print(f"step D={D} B={B}: steps vs one prefill, max |d state| / max |state|: GPU {e_gpu:.3g}, oracle {e_ref:.3g}")
     assert e_gpu <= 1.25 * e_ref + 1e-4
-
-
-def _smallm(a, w, out, M, N, K, epi, ws, bias, step=None):
-    p = _lib.GemmSmallMParams(A=a.data_ptr(), lda=K, W=w.data_ptr(), C=out.data_ptr(), ldc=out.shape[1], bias=bias.data_ptr(),
-                              residual=None, ldr=out.shape[1], M=M, N=N, K=K, epilogue=epi, workspace=ws.data_ptr(), workspace_bytes=ws.numel())
-    if step is not None:
-        fs, st, f = step
-        p.fir_state, p.state = fs.data_ptr(), st.data_ptr()
-        p.fir_w, p.fir_b, p.Dskip, p.poles, p.residues = f["w"].data_ptr(), f["b"].data_ptr(), f["D"].data_ptr(), f["p"].data_ptr(), f["r"].data_ptr()
-    _lib.check(_lib.lib().evo_gemm_smallm(C.byref(p), stream()), "evo_gemm_smallm")
-
-
-@pytest.mark.parametrize("M", [1, 16, 17, 64])
-def test_fused_step_epilogue_at_7b_width(M):
-    """EVO_EPI_HYENA_STEP on the 7B in-projection (N = 12288, K = 4096) over 8 carried steps.
-
-    The epilogue's step arithmetic is evo_hyena_step's, bit for bit: the fused kernel leaves the z it used, bf16(sum + bias),
-    in fir_state[..., 1], and evo_hyena_step on that z from the same states gives identical y, fir_state and state.
-
-    z itself is not always the z that stream-K EVO_EPI_BIAS stores.  A tile of three row groups gives 32 tiles instead of 96,
-    so the stream-K split cuts each tile's K sum at other k-blocks, and about 0.13 % of the fp32 sums round to another bf16
-    (measured on an H100 with 132 SMs).  So z is held to the stream-K GEMM bars against an fp64 sum, and to EVO_EPI_BIAS's own
-    worst error.  Where the two launches cut K at the same k-blocks, the paths are bit-identical end to end
-    (test_gpu_parity.py::test_decode_fused_hyena_step_epilogue_is_bit_identical, D = 256)."""
-    lib = _lib.lib()
-    D, H, N, K = 4096, 32, 12288, 4096
-    _, f = _filter_sd(D, seed=4)
-    torch.manual_seed(M)
-    w = (torch.randn(N, K, device=DEV) / 64).bfloat16()
-    bias = (torch.randn(N, device=DEV) * 0.2).bfloat16()
-    fs = torch.randn(M, 3 * D, 2, device=DEV).bfloat16()
-    st = torch.randn(M, D, 8, 2, device=DEV) * 0.5
-    ws1 = torch.zeros(lib.evo_gemm_smallm_workspace(M, N, K, _lib.EPI_BIAS), dtype=torch.uint8, device=DEV)
-    ws2 = torch.zeros(lib.evo_gemm_smallm_workspace(M, N, K, _lib.EPI_HYENA_STEP), dtype=torch.uint8, device=DEV)
-    zb = torch.empty(M, N, dtype=torch.bfloat16, device=DEV)
-    y1 = torch.empty(M, D, dtype=torch.bfloat16, device=DEV)
-    y2 = torch.full((M, D), float("nan"), dtype=torch.bfloat16, device=DEV)
-    for t in range(8):
-        a = (torch.randn(M, K, device=DEV) * 0.5).bfloat16()
-        fs1, st1 = fs.clone(), st.clone()
-        _smallm(a, w, y2, M, N, K, _lib.EPI_HYENA_STEP, ws2, bias, step=(fs, st, f))
-        z = fs[..., 1].contiguous()                              # the z the fused kernel computed
-        _step(z, y1, fs1, st1, f, M, D, H)
-        torch.cuda.synchronize()
-        assert torch.isfinite(y2.float()).all() and y2.float().abs().max() > 0
-        assert torch.equal(y1, y2), t
-        assert torch.equal(fs1, fs), t
-        assert torch.equal(st1, st), t
-        _smallm(a, w, zb, M, N, K, _lib.EPI_BIAS, ws1, bias)
-        torch.cuda.synchronize()
-        ref = a.double() @ w.double().T + bias.double()
-        scale = max(1.0, ref.abs().max().item())
-        # the bars of test_gemm_smallm_streamk_all_epilogues at K = 4096
-        assert maxerr(z, ref.bfloat16()) <= BF16_EPS * scale and (z == ref.bfloat16()).float().mean().item() > 0.90, t
-        assert maxerr(z, ref) <= maxerr(zb, ref) + BF16_EPS / 2 * scale, t
-        assert (z == zb).float().mean().item() > 0.99, t
 
 
 # ------------------------------------------------------------------ D. rejected calls

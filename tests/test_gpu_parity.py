@@ -515,7 +515,7 @@ def test_attention_kv_cache_form(variant):
 
 
 @pytest.mark.parametrize("Lc", [640, 600])
-def test_decode_attention_with_device_position(Lc):
+def test_decode_attention_with_device_position_advanced_by_counters(Lc):
     """evo_decode_qkv_prep + evo_decode_attn (position read from device memory) vs the oracle.  Lc = 640 takes the TMA-fed
     kernel (64-key tiles), Lc = 600 the per-thread-row kernel.  Cache rows past the position hold NaN (the reference
     allocates its cache with torch.empty, mha.py:349): they must not leak into the result."""
@@ -545,7 +545,7 @@ def test_decode_attention_with_device_position(Lc):
                                            1 / math.sqrt(128), _lib.ptr(ws), n, stream()))
             assert not torch.isnan(out.float()).any()
             assert maxerr(out, ref[:, pos]) <= 4 * BF16_EPS * max(1.0, ref.abs().max().item())
-    _lib.check(lib.evo_advance_position(_lib.ptr(posd), 3, stream()))
+    _lib.check(lib.evo_advance_counters(_lib.ptr(posd), None, 3, stream()))
     assert posd.item() == 602
 
 
@@ -689,41 +689,6 @@ def test_decode_streamk_pdl_paths_agree():
     assert maxerr(b, a) <= 0.03 * scale and maxerr(c, a) <= 0.03 * scale
     assert torch.equal(c, c2)
     assert torch.equal(b, c) and torch.equal(b, e) and torch.equal(b, f3) and torch.equal(b, f4)        # PDL and graph replay change scheduling only
-
-
-def test_decode_fused_hyena_step_epilogue_is_bit_identical():
-    """EVO_EPI_HYENA_STEP (engine.step_fir + step_iir inside the in-projection GEMM's epilogue) vs the two-launch path
-    (bias epilogue, then evo_hyena_step): logits AND the recurrent states after 40 steps, bit for bit; eager and graph replay."""
-    cfg, sd, m = _tiny()
-    torch.manual_seed(4)
-    ids = (torch.randint(0, 4, (3, 100)) * 3 + 65).to(DEV)
-
-    def run(fused, graph):
-        m.decode_fused_step, m.decode_graph, m._decode, m._loop = fused, graph, None, None
-        d = m.initialize_inference_params()
-        d["mha"].max_batch_size, d["mha"].max_seqlen = 3, 128
-        _, d = m(ids[:, :60], inference_params_dict=d)
-        d["mha"].seqlen_offset = d["hyena"].seqlen_offset = 60
-        outs = []
-        for t in range(60, 100):
-            s, d = m(ids[:, t:t + 1], inference_params_dict=d)
-            outs.append(s[:, 0].clone())
-            d["mha"].seqlen_offset += 1
-            d["hyena"].seqlen_offset += 1
-        return torch.stack(outs, 1), {k: v.clone() for k, v in d["hyena"].state_dict.items()}, {k: v.clone() for k, v in d["hyena"].fir_state_dict.items()}
-
-    saved = (m.decode_fused_step, m.decode_graph)
-    try:
-        a, sa, fa = run(False, False)
-        b, sb, fb = run(True, False)
-        c, sc, fc = run(True, True)
-    finally:
-        m.decode_fused_step, m.decode_graph = saved
-        m._decode = m._loop = None
-    assert torch.equal(a, b) and torch.equal(b, c)
-    for k in sa:
-        assert torch.equal(torch.view_as_real(sa[k]), torch.view_as_real(sb[k])) and torch.equal(torch.view_as_real(sb[k]), torch.view_as_real(sc[k]))
-        assert torch.equal(fa[k], fb[k]) and torch.equal(fb[k], fc[k])
 
 
 def test_public_api_scoring_and_generation():

@@ -56,7 +56,7 @@ def main():
     recs = []
 
     def emit(**kw):
-        kw.update(pdl=a.pdl, M=M, smem_kb=os.environ.get("EVO_B200_SMALLM_SMEM_KB"))
+        kw.update(pdl=a.pdl, M=M)
         print(json.dumps(kw), flush=True)
         recs.append(kw)
 
