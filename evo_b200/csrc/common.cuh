@@ -30,6 +30,82 @@ __device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
   bf162 t = __floats2bfloat162_rn(lo, hi);
   return *reinterpret_cast<uint32_t*>(&t);
 }
+__device__ __forceinline__ uint32_t ld_pair(const bf16* p) { return __ldg(reinterpret_cast<const unsigned int*>(p)); }
+
+// The reference's rounding chains (include/evo_b200.h states them per entry point), written once for every kernel that
+// applies them.  A "word" is a bf16 pair (columns n, n + 1) packed as pack_bf16 packs it; arguments named for a bf16 tensor
+// of the reference hold bf16 values.  Where a chain has a scalar and a word form, each keeps the order of operations its
+// callers compile best with; both round at the same points.
+
+// F.gelu (erf form).  erff stays IEEE: the library is built without --use_fast_math.
+__device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f)); }
+
+// ParallelGatedMLP, act(l1 x) * l2 x: bf16(gelu(l1)) * l2 of the bf16 linear outputs l1, l2; rounded on store.
+// gelu_gate_acc takes the fp32 sums a, b of the two linear layers instead: l1 = bf16(a), l2 = bf16(b).
+__device__ __forceinline__ float gelu_gate(float l1, float l2) { return rbf(gelu_erf(l1)) * l2; }
+__device__ __forceinline__ float gelu_gate_acc(float a, float b) { return rbf(gelu_erf(rbf(a))) * rbf(b); }
+
+// nn.Linear, then the residual add: C = bf16(bf16(acc + bias) + r).  Without a residual the rounding of acc + bias is the
+// store's; with one, acc + bias is rounded here and the sum is rounded on store.  linear_word reads the residual word through
+// load_resid() after the bias add; it is not called without RESID.
+template <bool BIAS, bool RESID>
+__device__ __forceinline__ float linear_out(float acc, float bias, float r) {
+  if constexpr (BIAS) acc += bias;
+  if constexpr (RESID) acc = rbf(acc) + r;
+  return acc;
+}
+template <bool BIAS, bool RESID, typename LoadResid>
+__device__ __forceinline__ uint32_t linear_word(float acc0, float acc1, uint32_t bias, LoadResid load_resid) {
+  if constexpr (BIAS) { acc0 += bf_lo(bias); acc1 += bf_hi(bias); }
+  if constexpr (RESID) { const uint32_t r = load_resid(); acc0 = rbf(acc0) + bf_lo(r); acc1 = rbf(acc1) + bf_hi(r); }
+  return pack_bf16(acc0, acc1);
+}
+// the residual add of linear_out on a word y that already holds bf16(acc + bias)
+__device__ __forceinline__ uint32_t resid_word(uint32_t y, uint32_t r) { return pack_bf16(bf_lo(y) + bf_lo(r), bf_hi(y) + bf_hi(r)); }
+
+// NeoX rotary (flash_attn apply_rotary) of head column c against c + 64, x and y their bf16 inputs, c and s the cos/sin table
+// entries of the token's position: fp32 arithmetic, one rounding (xr to column c, yr to c + 64).
+__device__ __forceinline__ void rope_rotate(float x, float y, float c, float s, bf16& xr, bf16& yr) {
+  xr = __float2bfloat16_rn(x * c - y * s);
+  yr = __float2bfloat16_rn(x * s + y * c);
+}
+// the same for columns (c, c + 1) against (c + 64, c + 65), cos/sin given as table words
+__device__ __forceinline__ void rope_words(float x0, float x1, float y0, float y1, uint32_t cw, uint32_t sw, uint32_t& o1, uint32_t& o2) {
+  const float cl = bf_lo(cw), ch = bf_hi(cw), sl = bf_lo(sw), sh = bf_hi(sw);
+  o1 = pack_bf16(x0 * cl - y0 * sl, x1 * ch - y1 * sh);
+  o2 = pack_bf16(x0 * sl + y0 * cl, x1 * sh + y1 * ch);
+}
+// the Wqkv projection with rotary (EVO_EPI_BIAS_ROPE): x = bf16(acc + bias), the reference's qkv tensor, for columns
+// (col, col + 1) and y for (col + 64, col + 65); then, when `rotate` (q and k heads), the rotation of head columns (c, c + 1)
+// with row l of the (positions, 64) cos/sin tables; else x and y as they are.
+__device__ __forceinline__ void bias_rope_words(float ax0, float ax1, float ay0, float ay1, const bf16* bias, int col, bool rotate,
+                                                const bf16* cos, const bf16* sin, long long l, int c, uint32_t& o1, uint32_t& o2) {
+  const uint32_t b1 = ld_pair(bias + col), b2 = ld_pair(bias + col + 64);
+  const float x0 = rbf(ax0 + bf_lo(b1)), x1 = rbf(ax1 + bf_hi(b1));
+  const float y0 = rbf(ay0 + bf_lo(b2)), y1 = rbf(ay1 + bf_hi(b2));
+  if (rotate) {
+    rope_words(x0, x1, y0, y1, ld_pair(cos + l * 64 + c), ld_pair(sin + l * 64 + c), o1, o2);
+  } else {
+    o1 = pack_bf16(x0, x1); o2 = pack_bf16(y0, y1);
+  }
+}
+
+// RMSNorm (layers.RMSNorm.forward, bf16 tensor ops): n = bf16(||x||), n = bf16(n * D^-1/2), n = bf16(n + eps), y = bf16(x / n),
+// out = bf16(scale * y).  rms_rinv takes the row's fp32 sum of squares and returns 1/n: the quotient is x * rcp(n) (one
+// reciprocal per row instead of an IEEE division per element, which made the kernels instruction-bound at ~50 % of HBM speed).
+// That is exact after the bf16 rounding: x and n have 8-bit significands, so x/n is either exactly representable or at least
+// 2^-17 (relative) away from every bf16 rounding midpoint (a 9-bit significand m with x = n*m would need x to have >= 9
+// significant bits), while x * rcp_rn(n) is within 2^-23 of x/n: both round to the same bf16.
+__device__ __forceinline__ float rms_rinv(float sumsq, float inv_sqrt_d, float eps) {
+  float n = rbf(sqrtf(sumsq));
+  n = rbf(n * inv_sqrt_d);
+  n = rbf(n + eps);
+  return __frcp_rn(n);
+}
+__device__ __forceinline__ uint32_t rms_word(uint32_t x, uint32_t scale, float rinv) {
+  const float y0 = rbf(bf_lo(x) * rinv), y1 = rbf(bf_hi(x) * rinv);
+  return pack_bf16(bf_lo(scale) * y0, bf_hi(scale) * y1);
+}
 
 // two-lane fp32 arithmetic with one IEEE round-to-nearest per lane (never contracted into an FMA)
 __device__ __forceinline__ float2 fadd2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }

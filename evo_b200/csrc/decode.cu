@@ -12,9 +12,7 @@ namespace {
 
 constexpr int HD = 128;
 
-__device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f)); }
-
-// out[m, g*128 + c] = bf16(gelu(t[m, g*256 + c])) * t[m, g*256 + 128 + c]   (t = [l1 | l2] interleaved GEMM output)
+// out[m, g*128 + c] = gelu_gate(t[m, g*256 + c], t[m, g*256 + 128 + c])   (t = [l1 | l2] interleaved GEMM output)
 __global__ void gelu_gate_kernel(const bf16* __restrict__ t, bf16* __restrict__ out, long long M, int ipad) {
   long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;      // (m, pair of columns)
   long long total = M * (ipad / 2);
@@ -24,8 +22,7 @@ __global__ void gelu_gate_kernel(const bf16* __restrict__ t, bf16* __restrict__ 
   int g = c2 / 128, c = c2 % 128;
   const uint32_t a = *reinterpret_cast<const uint32_t*>(t + m * 2 * ipad + g * 256 + c);
   const uint32_t b = *reinterpret_cast<const uint32_t*>(t + m * 2 * ipad + g * 256 + 128 + c);
-  float o0 = rbf(gelu_erf(bf_lo(a))) * bf_lo(b), o1 = rbf(gelu_erf(bf_hi(a))) * bf_hi(b);
-  *reinterpret_cast<uint32_t*>(out + m * ipad + c2) = pack_bf16(o0, o1);
+  *reinterpret_cast<uint32_t*>(out + m * ipad + c2) = pack_bf16(gelu_gate(bf_lo(a), bf_lo(b)), gelu_gate(bf_hi(a), bf_hi(b)));
 }
 
 // Rotary on element pair (i, i + 64) of q,k of row b, head h at position `pos`; k,v appended at cache row `row`.
@@ -37,9 +34,9 @@ __device__ __forceinline__ void qkv_prep_pair(bf16* __restrict__ qkv, bf16* __re
   const bf16* v = qkv + ((long long)(b * 3 + 2) * H + h) * HD;
   float q0 = __bfloat162float(q[i]), q1 = __bfloat162float(q[i + 64]);
   float k0 = __bfloat162float(k[i]), k1 = __bfloat162float(k[i + 64]);
-  bf16 kr0 = __float2bfloat16_rn(k0 * c - k1 * s), kr1 = __float2bfloat16_rn(k0 * s + k1 * c);
-  q[i] = __float2bfloat16_rn(q0 * c - q1 * s);
-  q[i + 64] = __float2bfloat16_rn(q0 * s + q1 * c);
+  bf16 kr0, kr1;
+  rope_rotate(k0, k1, c, s, kr0, kr1);
+  rope_rotate(q0, q1, c, s, q[i], q[i + 64]);
   k[i] = kr0; k[i + 64] = kr1;
   bf16* ck = cache + (((long long)b * max_seqlen + row) * 2 + 0) * H * HD + (long long)h * HD;
   bf16* cv = ck + (long long)H * HD;

@@ -34,14 +34,8 @@ extern "C" int evo_embed(const void* ids, int ids_are_i64, const void* table, vo
 }
 
 // ------------------------------------------------------------------ RMSNorm
-// One warp per row; the row stays in registers between the reduction and the scale.
-// Rounding points follow the reference's bf16 tensor ops (layers.RMSNorm.forward):
-//   n = bf16(||x||) ; n = bf16(n * D^-1/2) ; n = bf16(n + eps) ; y = bf16(x / n) ; out = bf16(scale * y)
-// The quotient is computed as x * rcp(n) (one reciprocal per row instead of 2*D/32 IEEE divisions per lane, which made the
-// kernel instruction-bound at ~50 % of HBM speed).  This is exact after the bf16 rounding: x and n have 8-bit
-// significands, so x/n is either exactly representable or at least 2^-17 (relative) away from every bf16 rounding
-// midpoint (a 9-bit significand m with x = n*m would need x to have >= 9 significant bits), while x * rcp_rn(n)
-// is within 2^-23 of x/n: both round to the same bf16.
+// One warp per row; the row stays in registers between the reduction and the scale.  The rounding chain is rms_rinv and
+// rms_word (common.cuh).
 template <int MAXV>
 __global__ void __launch_bounds__(256) rmsnorm_kernel(const uint4* __restrict__ x, const uint4* __restrict__ scale,
                                                       uint4* __restrict__ out, int64_t rows, int nvec_per_lane,
@@ -65,10 +59,7 @@ __global__ void __launch_bounds__(256) rmsnorm_kernel(const uint4* __restrict__ 
   }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
-  float n = rbf(sqrtf(ss));
-  n = rbf(n * inv_sqrt_d);
-  n = rbf(n + eps);
-  const float rinv = __frcp_rn(n);          // see the note above rmsnorm_kernel: bf16(x * (1/n)) == bf16(x / n) for bf16 x, n
+  const float rinv = rms_rinv(ss, inv_sqrt_d, eps);
   uint4* orow = out + row * row_vec;
 #pragma unroll
   for (int i = 0; i < MAXV; ++i) {
@@ -79,17 +70,14 @@ __global__ void __launch_bounds__(256) rmsnorm_kernel(const uint4* __restrict__ 
       uint4 o;
       uint32_t* ow = reinterpret_cast<uint32_t*>(&o);
 #pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        float y0 = rbf(bf_lo(w[j]) * rinv), y1 = rbf(bf_hi(w[j]) * rinv);
-        ow[j] = pack_bf16(bf_lo(sw[j]) * y0, bf_hi(sw[j]) * y1);
-      }
+      for (int j = 0; j < 4; ++j) ow[j] = rms_word(w[j], sw[j], rinv);
       orow[i * 32 + lane] = o;
     }
   }
 }
 
 // Few rows (decode step): one 256-thread CTA per row instead of one warp per row -- the row and the scale are fetched
-// by 8 warps at once (the warp-per-row kernel is a 5 us latency chain on 2 CTAs at 16 rows).  Same rounding chain.
+// by 8 warps at once (the warp-per-row kernel is a 5 us latency chain on 2 CTAs at 16 rows).
 __global__ void __launch_bounds__(256) rmsnorm_row_kernel(const uint4* __restrict__ x, const uint4* __restrict__ scale,
                                                           uint4* __restrict__ out, int row_vec, float inv_sqrt_d, float eps) {
   pdl_launch_dependents(); pdl_wait();
@@ -118,10 +106,7 @@ __global__ void __launch_bounds__(256) rmsnorm_row_kernel(const uint4* __restric
   float tot = 0.f;
 #pragma unroll
   for (int w = 0; w < 8; ++w) tot += red[w];
-  float n = rbf(sqrtf(tot));
-  n = rbf(n * inv_sqrt_d);
-  n = rbf(n + eps);
-  const float rinv = __frcp_rn(n);
+  const float rinv = rms_rinv(tot, inv_sqrt_d, eps);
   uint4* orow = out + (int64_t)blockIdx.x * row_vec;
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
@@ -132,10 +117,7 @@ __global__ void __launch_bounds__(256) rmsnorm_row_kernel(const uint4* __restric
       uint4 o;
       uint32_t* ow = reinterpret_cast<uint32_t*>(&o);
 #pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        float y0 = rbf(bf_lo(w[j]) * rinv), y1 = rbf(bf_hi(w[j]) * rinv);
-        ow[j] = pack_bf16(bf_lo(sw[j]) * y0, bf_hi(sw[j]) * y1);
-      }
+      for (int j = 0; j < 4; ++j) ow[j] = rms_word(w[j], sw[j], rinv);
       orow[idx] = o;
     }
   }
@@ -203,12 +185,7 @@ __global__ void rotary_qk_kernel(uint4* __restrict__ qkv, const uint4* __restric
   uint4 oa, ob;
   uint32_t *oaw = (uint32_t*)&oa, *obw = (uint32_t*)&ob;
 #pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    float x0l = bf_lo(aw[j]), x0h = bf_hi(aw[j]), x1l = bf_lo(bw[j]), x1h = bf_hi(bw[j]);
-    float cl = bf_lo(cw[j]), ch = bf_hi(cw[j]), sl = bf_lo(sw[j]), sh = bf_hi(sw[j]);
-    oaw[j] = pack_bf16(x0l * cl - x1l * sl, x0h * ch - x1h * sh);
-    obw[j] = pack_bf16(x0l * sl + x1l * cl, x0h * sh + x1h * ch);
-  }
+  for (int j = 0; j < 4; ++j) rope_words(bf_lo(aw[j]), bf_hi(aw[j]), bf_lo(bw[j]), bf_hi(bw[j]), cw[j], sw[j], oaw[j], obw[j]);
   base[c] = oa;
   base[c + vec_per_half] = ob;
 }

@@ -48,7 +48,6 @@ struct SmArgs {
   float* slots;                     // [2 * gridDim.x][R * Mb][128] fp32 partials
 };
 
-__device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f)); }
 // first k-block iteration of CTA c when `total` iterations are cut into `parts` contiguous ranges.  32-bit on purpose
 // (the host checks total * parts < 2^31): 64-bit division is a ~100-instruction subroutine and this sits in the tail.
 __device__ __forceinline__ uint32_t range_start(uint32_t c, uint32_t total, uint32_t parts) { return c * total / parts; }
@@ -78,14 +77,9 @@ __device__ __forceinline__ void finalize16(const SmArgs& g, long long n, int b0,
 #pragma unroll
   for (int j = 0; j < 16; ++j) {
     const int b = b0 + j;
-    float o;
-    if constexpr (EPI == EVO_EPI_GELU_GATE) {
-      o = rbf(gelu_erf(rbf(v0[j]))) * rbf(v1[j]);
-    } else {
-      o = v0[j];
-      if constexpr (EPI == EVO_EPI_BIAS || EPI == EVO_EPI_BIAS_RESID) o += bias;
-      if constexpr (EPI == EVO_EPI_BIAS_RESID || EPI == EVO_EPI_RESID) o = rbf(o) + rv[j];
-    }
+    const float o = EPI == EVO_EPI_GELU_GATE ? gelu_gate_acc(v0[j], v1[j])
+                                             : linear_out<EPI == EVO_EPI_BIAS || EPI == EVO_EPI_BIAS_RESID,
+                                                          EPI == EVO_EPI_BIAS_RESID || EPI == EVO_EPI_RESID>(v0[j], bias, rv[j]);
     if (b < g.M) g.C[(long long)b * g.ldc + n] = __float2bfloat16_rn(o);
   }
 }
@@ -312,18 +306,7 @@ int launch(const evo_gemm_smallm_params* p, cudaStream_t st) {
   static unsigned long long attr_done = 0;
   auto kern = gemm_smallm_kernel<EPI, MB>;
   { int rc_ = ensure_dyn_smem(kern, 227 * 1024, attr_done); if (rc_) return rc_; }
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(grid);
-  cfg.blockDim = dim3(NTHREADS);
-  cfg.dynamicSmemBytes = smem_bytes;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  if (pdl_level() >= 1) {
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = 1;
-  }
-  EVO_CUDA(cudaLaunchKernelEx(&cfg, kern, tmW, tmA, g));
+  EVO_CUDA(launch_pdl_at(1, kern, dim3(grid), dim3(NTHREADS), smem_bytes, st, tmW, tmA, g));
   return check_launch("evo_gemm_smallm");
 }
 

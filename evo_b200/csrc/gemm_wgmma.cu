@@ -10,8 +10,7 @@
 // BN = 256: the throughput tile (variants 0 and 1).  BN = 64: the small-M weight-streaming tile (variants 2 and 3;
 // variant 3 reads W tile-major, [N/64][K/64][64][64]), N/64 CTAs keep every SM pulling weights.
 //
-// Epilogues reproduce the reference's bf16 rounding points (nn.Linear output is rounded to
-// bf16 before the residual add / the gate): see include/evo_b200.h.
+// Epilogues reproduce the reference's bf16 rounding points (include/evo_b200.h) through the chain helpers of common.cuh.
 #include "common.cuh"
 #include "wgmma.cuh"
 #include "../../include/evo_b200.h"
@@ -67,8 +66,6 @@ struct GemmArgs {
 
 constexpr int EPI_LSE = 5;     // internal: scoring epilogue (evo_unembed_score); no C is written (EVO_EPI_BIAS_ROPE is 6)
 
-__device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f)); }
-
 // grouped rasterisation: GROUP_M row-blocks share the sweep over n so their A tiles stay in L2
 __device__ __forceinline__ void tile_coords(int tile, const GemmArgs& g, int& m_blk, int& n_blk) {
   const int major = g.raster_n ? g.n_blocks : g.m_blocks;     // the grouped dimension
@@ -91,20 +88,11 @@ __device__ __forceinline__ bf16* c_ptr(const GemmArgs& g, long long row, int col
   return g.c_peer[p] + (g.peer_row0 + row) * g.ldc + t * g.peer_inner + (rem - p * g.peer_inner);
 }
 
-__device__ __forceinline__ uint32_t ld_pair(const bf16* p) { return __ldg(reinterpret_cast<const unsigned int*>(p)); }
-
-// columns (col, col + 1) of one row: bias, then the bf16 rounding of the linear output, then the residual
-template <int EPI>
+// columns (col, col + 1) of one row
+template <bool BIAS, bool RESID>
 __device__ __forceinline__ void store_pair(const GemmArgs& g, long long row, int col, float v0, float v1) {
-  if constexpr (EPI == EVO_EPI_BIAS || EPI == EVO_EPI_BIAS_RESID) {
-    const uint32_t b = ld_pair(g.bias + col);
-    v0 += bf_lo(b); v1 += bf_hi(b);
-  }
-  if constexpr (EPI == EVO_EPI_BIAS_RESID || EPI == EVO_EPI_RESID) {
-    const uint32_t r = ld_pair(g.resid + row * g.ldr + col);
-    v0 = rbf(v0) + bf_lo(r); v1 = rbf(v1) + bf_hi(r);
-  }
-  *reinterpret_cast<uint32_t*>(c_ptr(g, row, col)) = pack_bf16(v0, v1);
+  *reinterpret_cast<uint32_t*>(c_ptr(g, row, col)) =
+      linear_word<BIAS, RESID>(v0, v1, BIAS ? ld_pair(g.bias + col) : 0u, [&] { return ld_pair(g.resid + row * g.ldr + col); });
 }
 
 // Quad exchange for full-sector stores.  Lane q of a quad holds bf16 pairs `lo` (columns 8i + 2q + {0, 1}) and `hi` (columns
@@ -142,6 +130,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tmA, const CUtensor
   using C_ = Cfg<BN, TMA_C>;
   static_assert(EPI != EVO_EPI_GELU_GATE || BN == BN_BIG, "the gate epilogue needs [l1 | l2] halves of a 256-column tile");
   static_assert(!TMA_C || (BN == BN_BIG && EPI != EPI_LSE), "TMA stores: the 256-column tile's C-writing epilogues");
+  constexpr bool BIAS = EPI == EVO_EPI_BIAS || EPI == EVO_EPI_BIAS_RESID;
   constexpr bool RESID = EPI == EVO_EPI_BIAS_RESID || EPI == EVO_EPI_RESID;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -237,9 +226,8 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tmA, const CUtensor
       // thread (warp, lane) holds rows r0 = 16 warp + lane/4 and r0 + 8 of its 64, columns 8i + 2 (lane%4) + {0, 1}
       const long long row0 = (long long)m_blk * BM + cw * 64 + warp * 16 + (lane >> 2);
       if constexpr (TMA_C) {
-        // The arithmetic and rounding points of the direct-store epilogues below, written as bf16 pairs into the staging;
-        // the TMA store clips rows >= M.  C may alias the residual: each element is read before its own store is issued.
-        constexpr bool BIAS = EPI == EVO_EPI_BIAS || EPI == EVO_EPI_BIAS_RESID;
+        // The direct-store epilogues below, written as bf16 pairs into the staging; the TMA store clips rows >= M.  C may
+        // alias the residual: each element is read before its own store is issued.
         constexpr int HALVES = EPI == EVO_EPI_GELU_GATE ? 1 : 2;      // the gate tile writes 128 columns
         const int rl0 = warp * 16 + (lane >> 2);
         if constexpr (!(RESID && STORE)) named_bar_sync(1 + cw, 128);  // after tid 0's wait for the previous stores
@@ -256,18 +244,9 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tmA, const CUtensor
 #pragma unroll
               for (int j = 0; j < 8; ++j) {      // columns c and c + 64 of the head in this half
                 const int i = 16 * hf + j, c = 8 * j + 2 * quad, col = n_blk * BN + 128 * hf + c;
-                const uint32_t b1 = ld_pair(g.bias + col), b2 = ld_pair(g.bias + col + 64);
-                const float x0 = rbf(acc[4 * i + 2 * h] + bf_lo(b1)), x1 = rbf(acc[4 * i + 2 * h + 1] + bf_hi(b1));
-                const float y0 = rbf(acc[4 * (i + 8) + 2 * h] + bf_lo(b2)), y1 = rbf(acc[4 * (i + 8) + 2 * h + 1] + bf_hi(b2));
                 uint32_t o1, o2;
-                if (rotate) {
-                  const uint32_t cw2 = ld_pair(g.rope_cos + l * 64 + c), sw2 = ld_pair(g.rope_sin + l * 64 + c);
-                  const float cl = bf_lo(cw2), ch = bf_hi(cw2), sl = bf_lo(sw2), sh = bf_hi(sw2);
-                  o1 = pack_bf16(x0 * cl - y0 * sl, x1 * ch - y1 * sh);
-                  o2 = pack_bf16(x0 * sl + y0 * cl, x1 * sh + y1 * ch);
-                } else {
-                  o1 = pack_bf16(x0, x1); o2 = pack_bf16(y0, y1);
-                }
+                bias_rope_words(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1], acc[4 * (i + 8) + 2 * h], acc[4 * (i + 8) + 2 * h + 1],
+                                g.bias, col, rotate, g.rope_cos, g.rope_sin, l, c, o1, o2);
                 *reinterpret_cast<uint32_t*>(buf + stage_off(rl, c)) = o1;
                 *reinterpret_cast<uint32_t*>(buf + stage_off(rl, c + 64)) = o2;
               }
@@ -276,20 +255,15 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tmA, const CUtensor
               for (int i = 0; i < BN / 16; ++i) {
                 const float a0 = rbf(acc[4 * i + 2 * h]), a1 = rbf(acc[4 * i + 2 * h + 1]);
                 const float b0 = rbf(acc[4 * (i + BN / 16) + 2 * h]), b1 = rbf(acc[4 * (i + BN / 16) + 2 * h + 1]);
-                *reinterpret_cast<uint32_t*>(buf + stage_off(rl, 8 * i + 2 * quad)) = pack_bf16(rbf(gelu_erf(a0)) * b0, rbf(gelu_erf(a1)) * b1);
+                *reinterpret_cast<uint32_t*>(buf + stage_off(rl, 8 * i + 2 * quad)) = pack_bf16(gelu_gate(a0, b0), gelu_gate(a1, b1));
               }
             } else {
 #pragma unroll
               for (int j = 0; j < 16; ++j) {
                 const int i = 16 * hf + j;
-                float v0 = acc[4 * i + 2 * h], v1 = acc[4 * i + 2 * h + 1];
-                if constexpr (BIAS) {
-                  const uint32_t b = ld_pair(g.bias + n_blk * BN + 8 * i + 2 * quad);
-                  v0 += bf_lo(b); v1 += bf_hi(b);
-                }
+                const uint32_t b = BIAS ? ld_pair(g.bias + n_blk * BN + 8 * i + 2 * quad) : 0u;
                 uint32_t* p = reinterpret_cast<uint32_t*>(buf + stage_off(rl, 8 * j + 2 * quad));
-                if constexpr (RESID) { const uint32_t r = *p; *p = pack_bf16(rbf(v0) + bf_lo(r), rbf(v1) + bf_hi(r)); }
-                else *p = pack_bf16(v0, v1);
+                *p = linear_word<BIAS, RESID>(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1], b, [&] { return *p; });
               }
             }
           }
@@ -331,9 +305,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tmA, const CUtensor
           if (quad == 0 && row < g.M) g.part[row * g.n_blocks + n_blk] = make_float4(mx, s, w, t_logit);
         }
       } else if constexpr (EPI == EVO_EPI_BIAS_ROPE && BN == BN_BIG) {
-        // columns c and c + 64 of one 128-wide head: x = bf16(acc + bias) (the reference's qkv tensor), then the NeoX rotation with
-        // the token's cos/sin row in fp32, one rounding on store -- the arithmetic of rotary_qk_kernel (elementwise.cu), which is
-        // flash_attn's apply_rotary (layers/rotary.py:382-416, mha.py:648).
+        // columns c and c + 64 of one 128-wide head
         const bool rotate = (long long)n_blk * BN < g.rope_cols;
         const int qc = quad_cols(quad);
 #pragma unroll
@@ -348,17 +320,8 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tmA, const CUtensor
 #pragma unroll
               for (int e = 0; e < 2; ++e) {
                 const int i = hc / 8 + i8 + e, c = 8 * (i8 + e) + 2 * quad, col = n_blk * BN + hc + c;
-                const uint32_t b1 = ld_pair(g.bias + col), b2 = ld_pair(g.bias + col + 64);
-                const float x0 = rbf(acc[4 * i + 2 * h] + bf_lo(b1)), x1 = rbf(acc[4 * i + 2 * h + 1] + bf_hi(b1));
-                const float y0 = rbf(acc[4 * (i + 8) + 2 * h] + bf_lo(b2)), y1 = rbf(acc[4 * (i + 8) + 2 * h + 1] + bf_hi(b2));
-                if (rotate) {
-                  const uint32_t cw2 = ld_pair(g.rope_cos + l * 64 + c), sw2 = ld_pair(g.rope_sin + l * 64 + c);
-                  const float cl = bf_lo(cw2), ch = bf_hi(cw2), sl = bf_lo(sw2), sh = bf_hi(sw2);
-                  o1[e] = pack_bf16(x0 * cl - y0 * sl, x1 * ch - y1 * sh);
-                  o2[e] = pack_bf16(x0 * sl + y0 * cl, x1 * sh + y1 * ch);
-                } else {
-                  o1[e] = pack_bf16(x0, x1); o2[e] = pack_bf16(y0, y1);
-                }
+                bias_rope_words(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1], acc[4 * (i + 8) + 2 * h], acc[4 * (i + 8) + 2 * h + 1],
+                                g.bias, col, rotate, g.rope_cos, g.rope_sin, l, c, o1[e], o2[e]);
               }
               const uint2 w1 = quad_pair(o1[0], o1[1], quad), w2 = quad_pair(o2[0], o2[1], quad);
               const int col = n_blk * BN + hc + 8 * i8 + qc;
@@ -367,7 +330,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tmA, const CUtensor
           }
         }
       } else if constexpr (EPI == EVO_EPI_GELU_GATE && BN == BN_BIG) {
-        // packed [l1 | l2] tile: output column n_blk * 128 + c = bf16(gelu(bf16(l1))) * bf16(l2)
+        // packed [l1 | l2] tile: output column n_blk * 128 + c from tile columns c and c + 128
         const int qc = quad_cols(quad);
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
@@ -379,17 +342,16 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tmA, const CUtensor
             for (int e = 0; e < 2; ++e) {
               const float a0 = rbf(acc[4 * (i + e) + 2 * h]), a1 = rbf(acc[4 * (i + e) + 2 * h + 1]);
               const float b0 = rbf(acc[4 * (i + e + BN / 16) + 2 * h]), b1 = rbf(acc[4 * (i + e + BN / 16) + 2 * h + 1]);
-              o[e] = pack_bf16(rbf(gelu_erf(a0)) * b0, rbf(gelu_erf(a1)) * b1);
+              o[e] = pack_bf16(gelu_gate(a0, b0), gelu_gate(a1, b1));
             }
             const uint2 w = quad_pair(o[0], o[1], quad);
             if (row < g.M) st_quad(c_ptr(g, row, n_blk * (BN / 2) + 8 * i + qc), w);
           }
         }
       } else if constexpr (BN == BN_BIG) {
-        // bias, then the bf16 rounding of the linear output (exact in the exchanged bf16 pairs), then the residual.  The residual
-        // of half a row is loaded ahead of its stores (one load latency per half row, not one per column pair); C may alias it,
-        // since every element is read before the same thread writes it.
-        constexpr bool BIAS = EPI == EVO_EPI_BIAS || EPI == EVO_EPI_BIAS_RESID;
+        // the linear output is rounded before the exchange (the exchanged bf16 pairs hold it exactly), the residual added after
+        // it.  The residual of half a row is loaded ahead of its stores (one load latency per half row, not one per column pair);
+        // C may alias it, since every element is read before the same thread writes it.
         const int qc = quad_cols(quad);
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
@@ -410,18 +372,11 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tmA, const CUtensor
               uint32_t o[2];
 #pragma unroll
               for (int e = 0; e < 2; ++e) {
-                float v0 = acc[4 * (2 * i + e) + 2 * h], v1 = acc[4 * (2 * i + e) + 2 * h + 1];
-                if constexpr (BIAS) {
-                  const uint32_t b = ld_pair(g.bias + n_blk * BN + 8 * (2 * i + e) + 2 * quad);
-                  v0 += bf_lo(b); v1 += bf_hi(b);
-                }
-                o[e] = pack_bf16(v0, v1);
+                const uint32_t b = BIAS ? ld_pair(g.bias + n_blk * BN + 8 * (2 * i + e) + 2 * quad) : 0u;
+                o[e] = linear_word<BIAS, false>(acc[4 * (2 * i + e) + 2 * h], acc[4 * (2 * i + e) + 2 * h + 1], b, 0);
               }
               uint2 w = quad_pair(o[0], o[1], quad);
-              if constexpr (RESID) {
-                w.x = pack_bf16(bf_lo(w.x) + bf_lo(r[j].x), bf_hi(w.x) + bf_hi(r[j].x));
-                w.y = pack_bf16(bf_lo(w.y) + bf_lo(r[j].y), bf_hi(w.y) + bf_hi(r[j].y));
-              }
+              if constexpr (RESID) { w.x = resid_word(w.x, r[j].x); w.y = resid_word(w.y, r[j].y); }
               if (live) st_quad(c_ptr(g, row, n_blk * BN + 16 * i + qc), w);
             }
           }
@@ -432,7 +387,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tmA, const CUtensor
           const long long row = row0 + 8 * h;
           if (row >= g.M) continue;
 #pragma unroll
-          for (int i = 0; i < BN / 8; ++i) store_pair<EPI>(g, row, n_blk * BN + 8 * i + 2 * quad, acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
+          for (int i = 0; i < BN / 8; ++i) store_pair<BIAS, RESID>(g, row, n_blk * BN + 8 * i + 2 * quad, acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
         }
       }
     }
@@ -504,12 +459,17 @@ int launch(const evo_gemm_params* p, cudaStream_t st, const long long* targets =
     if (env_g) g.group_m = std::max(1, atoi(env_g));
   }
   const int grid = std::min(g.m_blocks * g.n_blocks, device_sm_count());
+  // attr_done: one bit per device, a separate copy for each kernel instance
+  auto run = [&](auto kern, int smem_bytes, unsigned long long& attr_done, auto... args) {
+    if (int rc_ = ensure_dyn_smem(kern, smem_bytes, attr_done)) return rc_;
+    kern<<<grid, NTHREADS, smem_bytes, st>>>(args...);
+    return check_launch("evo_gemm");
+  };
   if constexpr (BN == BN_BIG && EPI != EPI_LSE) {
     // C by TMA stores unless it is peer-scattered; EVO_B200_GEMM_DIRECT_STORE=1 keeps the per-thread stores (the tests'
     // reference for the staged path)
     const char* env_d = getenv("EVO_B200_GEMM_DIRECT_STORE");
     if (p->n_c_peers == 0 && !(env_d && atoi(env_d))) {
-      using C_ = Cfg<BN, true>;
       constexpr bool RESID = EPI == EVO_EPI_BIAS_RESID || EPI == EVO_EPI_RESID;
       const uint64_t n_out = EPI == EVO_EPI_GELU_GATE ? p->N / 2 : p->N;
       CUtensorMap tmC, tmR;
@@ -517,18 +477,11 @@ int launch(const evo_gemm_params* p, cudaStream_t st, const long long* targets =
       if (RESID) { if ((rc = make_tmap_2d_bf16(&tmR, p->residual, n_out, (uint64_t)p->M, (uint64_t)p->ldr * 2, 64, 64, true))) return rc; }
       else tmR = tmC;
       static unsigned long long attr_done = 0;
-      auto kern = gemm_wgmma_tma_kernel<EPI>;
-      { int rc_ = ensure_dyn_smem(kern, C_::SMEM_BYTES, attr_done); if (rc_) return rc_; }
-      kern<<<grid, NTHREADS, C_::SMEM_BYTES, st>>>(tmA, tmB, tmC, tmR, g);
-      return check_launch("evo_gemm");
+      return run(gemm_wgmma_tma_kernel<EPI>, Cfg<BN, true>::SMEM_BYTES, attr_done, tmA, tmB, tmC, tmR, g);
     }
   }
-  using C_ = Cfg<BN>;
-  static unsigned long long attr_done = 0;     // one bit per device (the template instance has its own copy)
-  auto kern = gemm_wgmma_kernel<EPI, BN>;
-  { int rc_ = ensure_dyn_smem(kern, C_::SMEM_BYTES, attr_done); if (rc_) return rc_; }
-  kern<<<grid, NTHREADS, C_::SMEM_BYTES, st>>>(tmA, tmB, g);
-  return check_launch("evo_gemm");
+  static unsigned long long attr_done = 0;
+  return run(gemm_wgmma_kernel<EPI, BN>, Cfg<BN>::SMEM_BYTES, attr_done, tmA, tmB, g);
 }
 
 template <int BN>
