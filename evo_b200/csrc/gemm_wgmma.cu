@@ -239,8 +239,8 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tmA, const CUtensor
           for (int h = 0; h < 2; ++h) {
             const int rl = rl0 + 8 * h;
             if constexpr (EPI == EVO_EPI_BIAS_ROPE) {
-              const bool rotate = (long long)n_blk * BN < g.rope_cols;
-              const long long l = (row0 + 8 * h) % g.rope_L;
+              const bool rotate = (long long)n_blk * BN + 128 * hf < g.rope_cols;     // per 128-column head
+              const long long l = row0 + 8 * h < g.M ? (row0 + 8 * h) % g.rope_L : 0;   // rows >= M: any row in the tables
 #pragma unroll
               for (int j = 0; j < 8; ++j) {      // columns c and c + 64 of the head in this half
                 const int i = 16 * hf + j, c = 8 * j + 2 * quad, col = n_blk * BN + 128 * hf + c;
@@ -306,14 +306,14 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tmA, const CUtensor
         }
       } else if constexpr (EPI == EVO_EPI_BIAS_ROPE && BN == BN_BIG) {
         // columns c and c + 64 of one 128-wide head
-        const bool rotate = (long long)n_blk * BN < g.rope_cols;
         const int qc = quad_cols(quad);
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           const long long row = row0 + 8 * h;      // rows >= M (a ragged last block) compute and exchange, but store nothing
-          const long long l = row % g.rope_L;
+          const long long l = row < g.M ? row % g.rope_L : 0;   // and read table row 0: the tables need only cover rows < M
 #pragma unroll
           for (int hc = 0; hc < BN; hc += 128) {
+            const bool rotate = (long long)n_blk * BN + hc < g.rope_cols;             // per 128-column head
 #pragma unroll
             for (int i8 = 0; i8 < 8; i8 += 2) {
               uint32_t o1[2], o2[2];
