@@ -33,6 +33,10 @@ class GemmSmallMParams(C.Structure):
                 ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t)]
 
 
+class GemmSmallMFp8Params(C.Structure):
+    _fields_ = [("base", GemmSmallMParams), ("W_exp", C.c_void_p)]
+
+
 class HyenaParams(C.Structure):
     _fields_ = [("z", C.c_void_p), ("y", C.c_void_p), ("fir_w", C.c_void_p), ("fir_b", C.c_void_p), ("Dskip", C.c_void_p),
                 ("poles", C.c_void_p), ("residues", C.c_void_p),
@@ -114,6 +118,9 @@ SIGNATURES = {
     "evo_gemm": (C.c_int, [C.POINTER(GemmParams), C.c_void_p]),
     "evo_gemm_smallm_workspace": (C.c_size_t, [C.c_int64, C.c_int64, C.c_int64, C.c_int]),
     "evo_gemm_smallm": (C.c_int, [C.POINTER(GemmSmallMParams), C.c_void_p]),
+    "evo_fp8_weight_bytes": (C.c_size_t, [C.c_int64, C.c_int64, C.c_int]),
+    "evo_fp8_quantize_rows": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "evo_gemm_smallm_fp8": (C.c_int, [C.POINTER(GemmSmallMFp8Params), C.c_void_p]),
     "evo_set_pdl": (C.c_int, [C.c_int]),
     "evo_hyena_fwd_workspace": (C.c_size_t, [C.POINTER(HyenaParams)]),
     "evo_hyena_fwd": (C.c_int, [C.POINTER(HyenaParams), C.c_void_p, C.c_size_t, C.c_void_p]),

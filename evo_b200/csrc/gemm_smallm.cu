@@ -17,11 +17,21 @@
 // column, 16 batch values per pass; the two warpgroups take alternate 16-row batch chunks).
 // EVO_EPI_GELU_GATE: a tile is 256 packed rows [l1 | l2] (two MMA row groups), the epilogue thread holds l1[b] and
 // l2[b] of its column: gelu(l1)*l2 is fused.
+//
+// FP8 weights (evo_gemm_smallm_fp8, template flag FP8): W is stored as E4M3 q[n, k] with a power-of-two scale 2^e[n] per row,
+// W'[n, k] = q[n, k] 2^e[n], and the kernel streams q (one byte per weight) instead of the bf16 W'.  Only the path of the W operand
+// changes: one 1-D bulk copy per stage of a block laid out in the order of the wgmma A register fragments (the FP8 decode layout below), two
+// 16-byte shared loads per thread and k-block, an exact E4M3 -> bf16 conversion, and wgmma with A from registers.  The cut rule,
+// the grid, the fix-up order, the PDL prefetch and finalize16 are the bf16 kernel's; the scale 2^e[n] multiplies the fp32 sum of
+// column n once, after the fix-up's slot sum and before the epilogue.  A power-of-two scale commutes exactly with every fp32
+// partial sum (no under- or overflow at weight magnitudes), so the output is bit-identical to evo_gemm_smallm on W'.
 #include "common.cuh"
 #include "wgmma.cuh"
 #include "../../include/evo_b200.h"
+#include <cuda_fp8.h>
 #include <algorithm>
 #include <cmath>
+#include <cstring>
 
 using namespace evo;
 
@@ -46,7 +56,29 @@ struct SmArgs {
   int n_stages;
   int* counters;                    // [n_tiles], zero between launches
   float* slots;                     // [2 * gridDim.x][R * Mb][128] fp32 partials
+  const uint8_t* Wq;                // FP8 form: E4M3 weights in the FP8 decode layout
+  const int8_t* Wexp;               // FP8 form: (N) row exponents
 };
+
+// FP8 decode layout.  One contiguous block of 128 x 64 bytes per (tile, row group r, k-block) in iteration order (tile, k-block,
+// r), so a CTA's stream-K range is one contiguous run of DRAM.  Inside a block, consumer thread t of warpgroup cw (W rows
+// cw*64 + 16*(t/32) + (t%32)/4 [+8]) owns 32 bytes: its wgmma A fragments for the four k16 steps, split into two 16-byte halves
+// (k16 steps {0,1} and {2,3}) that lie 512 bytes apart, so that each quarter-warp's 16-byte loads cover 128 contiguous bytes
+// (no bank conflict).  Byte order inside a half: k16 step, fragment register a[0..3], low k of the pair first.  fp8_quantize_kernel
+// writes it (and is its one definition); the model's fp8_layout() is the host reference.
+constexpr int FP8_BLOCK = WROWS * BK;
+
+// four E4M3 values (bytes 0..3) -> two bf16 pairs: exact (f16 holds every E4M3 value as a normal number or zero, and bf16 every f16
+// with a 4-bit significand in E4M3's exponent range)
+__device__ __forceinline__ void e4m3x4_to_bf16x2(uint32_t v, uint32_t& lo, uint32_t& hi) {
+  uint32_t h0, h1;
+  asm("{\n\t.reg .b16 a, b;\n\tmov.b32 {a, b}, %2;\n\t"
+      "cvt.rn.f16x2.e4m3x2 %0, a;\n\tcvt.rn.f16x2.e4m3x2 %1, b;\n\t}\n" : "=r"(h0), "=r"(h1) : "r"(v));
+  const float2 f0 = __half22float2(*reinterpret_cast<const __half2*>(&h0)), f1 = __half22float2(*reinterpret_cast<const __half2*>(&h1));
+  lo = __byte_perm(__float_as_uint(f0.x), __float_as_uint(f0.y), 0x7632);
+  hi = __byte_perm(__float_as_uint(f1.x), __float_as_uint(f1.y), 0x7632);
+}
+__device__ __forceinline__ float pow2f(int e) { return __int_as_float((e + 127) << 23); }   // e in [-126, 127]
 
 // first k-block iteration of CTA c when `total` iterations are cut into `parts` contiguous ranges.  32-bit on purpose
 // (the host checks total * parts < 2^31): 64-bit division is a ~100-instruction subroutine and this sits in the tail.
@@ -94,13 +126,21 @@ __device__ __forceinline__ void wgmma_ss_n(float (&d)[MB / 2], uint64_t da, uint
   else wgmma_m64n64k16_ss(d, da, db, scale_d);
 }
 
-template <int EPI, int MB>
+template <int MB>
+__device__ __forceinline__ void wgmma_rs_n(float (&d)[MB / 2], const uint32_t (&a)[4], uint64_t db, int scale_d) {
+  if constexpr (MB == 16) wgmma_m64n16k16_rs(d, a, db, scale_d);
+  else if constexpr (MB == 32) wgmma_m64n32k16_rs(d, a, db, scale_d);
+  else if constexpr (MB == 48) wgmma_m64n48k16_rs(d, a, db, scale_d);
+  else wgmma_m64n64k16_rs(d, a, db, scale_d);
+}
+
+template <int EPI, int MB, bool FP8 = false>
 __global__ void __launch_bounds__(NTHREADS, 1)
 gemm_smallm_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmA, const SmArgs g) {
   constexpr int R = RowGroups<EPI>::R;                         // MMA row groups per tile
   constexpr int WBOX = R == 2 ? 2 * WROWS : WROWS;             // W rows per TMA box (a box dimension is at most 256)
   constexpr int NBOX = R * WROWS / WBOX;
-  constexpr int W_STAGE = R * WROWS * BK * 2;
+  constexpr int W_STAGE = FP8 ? R * FP8_BLOCK : R * WROWS * BK * 2;
   constexpr int A_STAGE = MB * BK * 2;
   constexpr int ACC_COLS = R * MB;                             // fp32 columns of one accumulator
   extern __shared__ __align__(1024) uint8_t smem[];
@@ -117,7 +157,8 @@ gemm_smallm_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constan
   if ((smem_u32(smem) & 1023u) != 0) __trap();
 
   if (threadIdx.x == 0) {
-    tma_prefetch_desc(&tmW); tma_prefetch_desc(&tmA);
+    if constexpr (!FP8) tma_prefetch_desc(&tmW);
+    tma_prefetch_desc(&tmA);
     for (int i = 0; i < MAXST; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], CONSUMER_WARPS); }
     fence_barrier_init();
   }
@@ -137,8 +178,12 @@ gemm_smallm_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constan
       int tile = tile_b, kb = kb_b;
       for (int i = 0; i < pre; ++i) {                         // weights first: they do not depend on the previous kernel
         mbar_arrive_expect_tx(&full[i], STAGE_TX);
+        if constexpr (FP8) {
+          bulk_load(smW + i * W_STAGE, g.Wq + (size_t)(it_begin + i) * W_STAGE, W_STAGE, &full[i]);
+        } else {
 #pragma unroll
-        for (int bx = 0; bx < NBOX; ++bx) tma_load_2d(smW + i * W_STAGE + bx * (WBOX * BK * 2), &tmW, &full[i], kb * BK, tile * (R * WROWS) + bx * WBOX);
+          for (int bx = 0; bx < NBOX; ++bx) tma_load_2d(smW + i * W_STAGE + bx * (WBOX * BK * 2), &tmW, &full[i], kb * BK, tile * (R * WROWS) + bx * WBOX);
+        }
         if (++kb == KB) { kb = 0; ++tile; }
       }
       pdl_wait();
@@ -151,8 +196,12 @@ gemm_smallm_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constan
       for (int i = pre; i < n_it; ++i) {
         mbar_wait(&empty[stage], phase ^ 1);
         mbar_arrive_expect_tx(&full[stage], STAGE_TX);
+        if constexpr (FP8) {
+          bulk_load(smW + stage * W_STAGE, g.Wq + (size_t)(it_begin + i) * W_STAGE, W_STAGE, &full[stage]);
+        } else {
 #pragma unroll
-        for (int bx = 0; bx < NBOX; ++bx) tma_load_2d(smW + stage * W_STAGE + bx * (WBOX * BK * 2), &tmW, &full[stage], kb * BK, tile * (R * WROWS) + bx * WBOX);
+          for (int bx = 0; bx < NBOX; ++bx) tma_load_2d(smW + stage * W_STAGE + bx * (WBOX * BK * 2), &tmW, &full[stage], kb * BK, tile * (R * WROWS) + bx * WBOX);
+        }
         tma_load_2d(smA + stage * A_STAGE, &tmA, &full[stage], kb * BK, 0);
         if (++kb == KB) { kb = 0; ++tile; }
         if (++stage == NST) { stage = 0; phase ^= 1; }
@@ -177,16 +226,37 @@ gemm_smallm_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constan
       for (int kb = k0; kb < k1; ++kb) {
         mbar_wait(&full[stage], phase);
         const uint32_t b0 = smem_u32(smA + stage * A_STAGE);
-        wgmma_fence();
+        if constexpr (FP8) {
+          uint32_t af[R][BK / UK][4];
 #pragma unroll
-        for (int r = 0; r < R; ++r) {
-          const uint32_t a0 = smem_u32(smW + stage * W_STAGE + r * (WROWS * BK * 2) + cw * 64 * 128);
+          for (int r = 0; r < R; ++r) {
+            const uint8_t* q = smW + stage * W_STAGE + r * FP8_BLOCK + cw * 4096 + warp * 1024 + lane * 16;
+            const uint4 h0 = *reinterpret_cast<const uint4*>(q), h1 = *reinterpret_cast<const uint4*>(q + 512);
+            e4m3x4_to_bf16x2(h0.x, af[r][0][0], af[r][0][1]); e4m3x4_to_bf16x2(h0.y, af[r][0][2], af[r][0][3]);
+            e4m3x4_to_bf16x2(h0.z, af[r][1][0], af[r][1][1]); e4m3x4_to_bf16x2(h0.w, af[r][1][2], af[r][1][3]);
+            e4m3x4_to_bf16x2(h1.x, af[r][2][0], af[r][2][1]); e4m3x4_to_bf16x2(h1.y, af[r][2][2], af[r][2][3]);
+            e4m3x4_to_bf16x2(h1.z, af[r][3][0], af[r][3][1]); e4m3x4_to_bf16x2(h1.w, af[r][3][2], af[r][3][3]);
+          }
+          wgmma_fence();
 #pragma unroll
-          for (int k = 0; k < BK / UK; ++k)
-            wgmma_ss_n<MB>(acc[r], wgmma_desc_k_sw128(a0 + k * 32), wgmma_desc_k_sw128(b0 + k * 32), (kb != k0 || k != 0));
+          for (int r = 0; r < R; ++r)
+#pragma unroll
+            for (int k = 0; k < BK / UK; ++k) wgmma_rs_n<MB>(acc[r], af[r][k], wgmma_desc_k_sw128(b0 + k * 32), (kb != k0 || k != 0));
+        } else {
+          wgmma_fence();
+#pragma unroll
+          for (int r = 0; r < R; ++r) {
+            const uint32_t a0 = smem_u32(smW + stage * W_STAGE + r * (WROWS * BK * 2) + cw * 64 * 128);
+#pragma unroll
+            for (int k = 0; k < BK / UK; ++k)
+              wgmma_ss_n<MB>(acc[r], wgmma_desc_k_sw128(a0 + k * 32), wgmma_desc_k_sw128(b0 + k * 32), (kb != k0 || k != 0));
+          }
         }
         wgmma_commit();
-        wgmma_wait<1>();
+        // FP8: the next k-block's conversion rewrites the A fragment registers, which an unfinished register-A wgmma may
+        // still read (undefined in PTX; at the gate's register pressure it gave wrong and launch-dependent sums): wait for it
+        if constexpr (FP8) wgmma_wait<0>();
+        else wgmma_wait<1>();
         if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
         prev = stage;
         if (++stage == NST) { stage = 0; phase ^= 1; }
@@ -209,6 +279,11 @@ gemm_smallm_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constan
       const long long n = (long long)tile * WROWS + row;      // output column (gate: of the N/2-wide output)
       float bias = 0.f;
       if constexpr (EPI == EVO_EPI_BIAS || EPI == EVO_EPI_BIAS_RESID) bias = __bfloat162float(g.bias[n]);
+      float s0 = 1.f, s1 = 1.f;                               // FP8: 2^e of the column's W row (gate: of its l1 and l2 rows)
+      if constexpr (FP8) {
+        s0 = pow2f(g.Wexp[(long long)tile * R * WROWS + row]);
+        if constexpr (R >= 2) s1 = pow2f(g.Wexp[(long long)tile * R * WROWS + WROWS + row]);
+      }
       if (whole) {
         for (int c = cw * 16; c < MB; c += 32) {
           float rv[16], v0[16], v1[16];
@@ -217,6 +292,7 @@ gemm_smallm_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constan
           for (int j = 0; j < 16; ++j) {
             v0[j] = stg[(c + j) * STG_LD + row];
             v1[j] = R >= 2 ? stg[(MB + c + j) * STG_LD + row] : 0.f;
+            if constexpr (FP8) { v0[j] *= s0; v1[j] *= s1; }
           }
           finalize16<EPI>(g, n, c, bias, rv, v0, v1);
         }
@@ -267,6 +343,10 @@ gemm_smallm_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constan
                 }
               }
             }
+            if constexpr (FP8) {
+#pragma unroll
+              for (int j = 0; j < 16; ++j) { v0[j] *= s0; v1[j] *= s1; }
+            }
             finalize16<EPI>(g, n, c, bias, rv, v0, v1);
           }
           if (threadIdx.x == 128) g.counters[tile] = 0;      // self-cleaning for the next launch
@@ -278,19 +358,21 @@ gemm_smallm_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constan
   }
 }
 
-template <int EPI, int MB>
-int launch(const evo_gemm_smallm_params* p, cudaStream_t st) {
+template <int EPI, int MB, bool FP8>
+int launch(const evo_gemm_smallm_params* p, const void* w_exp, cudaStream_t st) {
   constexpr int R = RowGroups<EPI>::R;
   CUtensorMap tmW, tmA;
   int rc;
-  if ((rc = make_tmap_2d_bf16(&tmW, p->W, (uint64_t)p->K, (uint64_t)p->N, (uint64_t)p->K * 2, BK, R == 2 ? 2 * WROWS : WROWS, true))) return rc;
+  if constexpr (FP8) memset(&tmW, 0, sizeof(tmW));            // the FP8 form streams W by 1-D bulk copies
+  else if ((rc = make_tmap_2d_bf16(&tmW, p->W, (uint64_t)p->K, (uint64_t)p->N, (uint64_t)p->K * 2, BK, R == 2 ? 2 * WROWS : WROWS, true))) return rc;
   if ((rc = make_tmap_2d_bf16(&tmA, p->A, (uint64_t)p->K, (uint64_t)p->M, (uint64_t)p->lda * 2, BK, (uint32_t)MB, true))) return rc;
   SmArgs g;
+  g.Wq = (const uint8_t*)p->W; g.Wexp = (const int8_t*)w_exp;
   g.C = (bf16*)p->C; g.ldc = p->ldc; g.bias = (const bf16*)p->bias; g.resid = (const bf16*)p->residual; g.ldr = p->ldr;
   g.M = (int)p->M; g.Mb = MB;
   g.n_tiles = (int)(p->N / (R * WROWS));
   g.KB = (int)(p->K / BK);
-  const int stage_bytes = R * WROWS * BK * 2 + MB * BK * 2;
+  const int stage_bytes = (FP8 ? R * FP8_BLOCK : R * WROWS * BK * 2) + MB * BK * 2;
   const int tail = R * MB * STG_LD * 4 + 2 * MAXST * 8 + 16;
   const int budget = std::min(RING_BYTES, 227 * 1024 - tail);
   g.n_stages = std::max(2, std::min(MAXST, budget / stage_bytes));
@@ -304,19 +386,116 @@ int launch(const evo_gemm_smallm_params* p, cudaStream_t st) {
   g.counters = (int*)p->workspace;
   g.slots = (float*)((uint8_t*)p->workspace + 16384);
   static unsigned long long attr_done = 0;
-  auto kern = gemm_smallm_kernel<EPI, MB>;
+  auto kern = gemm_smallm_kernel<EPI, MB, FP8>;
   { int rc_ = ensure_dyn_smem(kern, 227 * 1024, attr_done); if (rc_) return rc_; }
   EVO_CUDA(launch_pdl_at(1, kern, dim3(grid), dim3(NTHREADS), smem_bytes, st, tmW, tmA, g));
-  return check_launch("evo_gemm_smallm");
+  return check_launch(FP8 ? "evo_gemm_smallm_fp8" : "evo_gemm_smallm");
 }
 
-template <int EPI>
-int launch_mb(const evo_gemm_smallm_params* p, cudaStream_t st) {
+template <int EPI, bool FP8>
+int launch_mb(const evo_gemm_smallm_params* p, const void* w_exp, cudaStream_t st) {
   switch ((p->M + 15) / 16) {
-    case 1: return launch<EPI, 16>(p, st);
-    case 2: return launch<EPI, 32>(p, st);
-    case 3: return launch<EPI, 48>(p, st);
-    default: return launch<EPI, 64>(p, st);
+    case 1: return launch<EPI, 16, FP8>(p, w_exp, st);
+    case 2: return launch<EPI, 32, FP8>(p, w_exp, st);
+    case 3: return launch<EPI, 48, FP8>(p, w_exp, st);
+    default: return launch<EPI, 64, FP8>(p, w_exp, st);
+  }
+}
+
+// the argument checks of both forms, under the entry point's name
+int check_smallm(const char* what, const evo_gemm_smallm_params* p) {
+  EVO_REQUIRE(p->M >= 0 && p->M <= MAX_MB, "%s: M (%lld) must be in [0, %d]", what, (long long)p->M, MAX_MB);
+  EVO_REQUIRE(p->N > 0 && p->K > 0 && p->K % BK == 0, "%s: K (%lld) must be a positive multiple of %d", what, (long long)p->K, BK);
+  EVO_REQUIRE(p->N % 256 == 0 && p->N / WROWS <= 4096, "%s: N (%lld) must be a multiple of 256 (and <= 524288)", what, (long long)p->N);
+  EVO_REQUIRE(p->lda % 8 == 0, "%s: lda must be a multiple of 8 elements", what);
+  EVO_REQUIRE(((uintptr_t)p->A % 16) == 0 && ((uintptr_t)p->W % 16) == 0, "%s: A and W must be 16-byte aligned", what);
+  if (p->epilogue == EVO_EPI_BIAS || p->epilogue == EVO_EPI_BIAS_RESID) EVO_REQUIRE(p->bias != nullptr, "%s: bias epilogue without bias", what);
+  if (p->epilogue == EVO_EPI_RESID || p->epilogue == EVO_EPI_BIAS_RESID) EVO_REQUIRE(p->residual != nullptr, "%s: residual epilogue without residual", what);
+  return 0;
+}
+
+template <bool FP8>
+int dispatch(const char* what, const evo_gemm_smallm_params* p, const void* w_exp, cudaStream_t st) {
+  switch (p->epilogue) {
+    case EVO_EPI_NONE: return launch_mb<EVO_EPI_NONE, FP8>(p, w_exp, st);
+    case EVO_EPI_BIAS: return launch_mb<EVO_EPI_BIAS, FP8>(p, w_exp, st);
+    case EVO_EPI_BIAS_RESID: return launch_mb<EVO_EPI_BIAS_RESID, FP8>(p, w_exp, st);
+    case EVO_EPI_RESID: return launch_mb<EVO_EPI_RESID, FP8>(p, w_exp, st);
+    case EVO_EPI_GELU_GATE: return launch_mb<EVO_EPI_GELU_GATE, FP8>(p, w_exp, st);
+  }
+  set_error("%s: unknown epilogue %d", what, p->epilogue);
+  return -1;
+}
+
+// ---- quantizer of the FP8 decode weights
+// e[n] = ceil(log2(amax_n / 448)), at least -124 (so that every q 2^e is a bf16 number and 2^e a normal fp32 one); 0 for an all-zero
+// row.  amax = m 2^p with m in [0.5, 1) and 448 = 0.875 2^9: amax / 448 lies in (2^(p-10), 2^(p-9)] when m <= 0.875.
+__global__ void fp8_row_exp_kernel(const bf16* __restrict__ W, int K, int8_t* __restrict__ w_exp, int* status) {
+  const long long n = blockIdx.x;
+  float amax = 0.f;
+  bool bad = false;
+  for (int k = threadIdx.x * 8; k < K; k += blockDim.x * 8) {
+    const uint4 v = *reinterpret_cast<const uint4*>(W + n * K + k);
+    const uint32_t w4[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const float a = fabsf(bf_lo(w4[j])), b = fabsf(bf_hi(w4[j]));
+      bad |= !(a <= 3.0e38f) || !(b <= 3.0e38f);
+      amax = fmaxf(amax, fmaxf(a, b));
+    }
+  }
+  __shared__ float red[32];
+  __shared__ int red_bad[32];
+  for (int o = 16; o; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+  bad = __any_sync(0xffffffffu, bad);
+  if ((threadIdx.x & 31) == 0) { red[threadIdx.x >> 5] = amax; red_bad[threadIdx.x >> 5] = bad; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int i = 1; i < (int)(blockDim.x >> 5); ++i) { amax = fmaxf(amax, red[i]); bad |= red_bad[i] != 0; }
+    int e = 0;
+    if (amax > 0.f) {
+      int p;
+      const float m = frexpf(amax, &p);
+      e = max(m <= 0.875f ? p - 9 : p - 8, -124);
+    }
+    w_exp[n] = (int8_t)e;
+    if (bad) atomicOr(status, 1);
+  }
+}
+
+// one thread per 16 bytes of the layout: q = E4M3(w 2^-e) (round to nearest even; |w 2^-e| <= 448), W' = q 2^e over w in place.
+// Does nothing when any weight of the matrix was not finite.
+__global__ void fp8_quantize_kernel(bf16* W, long long K, int KB, int R, const int8_t* __restrict__ w_exp, uint8_t* __restrict__ q,
+                                    const int* status, long long n_chunks) {
+  if (*status) return;
+  for (long long c = blockIdx.x * (long long)blockDim.x + threadIdx.x; c < n_chunks; c += (long long)gridDim.x * blockDim.x) {
+    // chunk c = (block of R*8192 bytes, r, warpgroup, warp, half, lane), the FP8 decode layout
+    const long long blk = c / (R * 512);
+    int rem = (int)(c - blk * R * 512);
+    const int r = rem / 512, cw = (rem / 256) % 2, warp = (rem / 64) % 4, h = (rem / 32) % 2, lane = rem % 32;
+    const long long tile = blk / KB;
+    const int kb = (int)(blk - tile * KB);
+    uint32_t out[4];
+#pragma unroll
+    for (int b = 0; b < 16; b += 2) {
+      const int ks = 2 * h + b / 8, reg = (b % 8) / 2;
+      const long long n = tile * R * WROWS + r * WROWS + cw * 64 + warp * 16 + (reg % 2) * 8 + lane / 4;
+      const long long k = (long long)kb * BK + ks * UK + (reg / 2) * 8 + (lane % 4) * 2;
+      const int e = w_exp[n];
+      bf16* wp = W + n * K + k;
+      const uint32_t wv = *reinterpret_cast<const uint32_t*>(wp);
+      const float inv = pow2f(-e), sc = pow2f(e);
+      __nv_fp8x2_storage_t q2 = __nv_cvt_float2_to_fp8x2(make_float2(bf_lo(wv) * inv, bf_hi(wv) * inv), __NV_SATFINITE, __NV_E4M3);
+      // the conversion returns +0 for a negative value that rounds to zero; round to nearest keeps the sign (-0)
+      if ((q2 & 0x007f) == 0 && (wv & 0x8000u)) q2 |= 0x0080;
+      if ((q2 & 0x7f00) == 0 && (wv & 0x80000000u)) q2 |= 0x8000;
+      const __half2_raw hr = __nv_cvt_fp8x2_to_halfraw2(q2, __NV_E4M3);
+      const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&hr));
+      *reinterpret_cast<uint32_t*>(wp) = pack_bf16(f.x * sc, f.y * sc);
+      const uint32_t q16 = (uint32_t)q2;
+      if (b % 4 == 0) out[b / 4] = q16; else out[b / 4] |= q16 << 16;
+    }
+    *reinterpret_cast<uint4*>(q + c * 16) = make_uint4(out[0], out[1], out[2], out[3]);
   }
 }
 
@@ -331,21 +510,41 @@ extern "C" size_t evo_gemm_smallm_workspace(int64_t M, int64_t N, int64_t K, int
 }
 
 extern "C" int evo_gemm_smallm(const evo_gemm_smallm_params* p, void* stream) {
-  EVO_REQUIRE(p->M >= 0 && p->M <= MAX_MB, "evo_gemm_smallm: M (%lld) must be in [0, %d]", (long long)p->M, MAX_MB);
-  EVO_REQUIRE(p->N > 0 && p->K > 0 && p->K % BK == 0, "evo_gemm_smallm: K (%lld) must be a positive multiple of %d", (long long)p->K, BK);
-  EVO_REQUIRE(p->N % 256 == 0 && p->N / WROWS <= 4096, "evo_gemm_smallm: N (%lld) must be a multiple of 256 (and <= 524288)", (long long)p->N);
-  EVO_REQUIRE(p->lda % 8 == 0, "evo_gemm_smallm: lda must be a multiple of 8 elements");
-  EVO_REQUIRE(((uintptr_t)p->A % 16) == 0 && ((uintptr_t)p->W % 16) == 0, "evo_gemm_smallm: A and W must be 16-byte aligned");
-  if (p->epilogue == EVO_EPI_BIAS || p->epilogue == EVO_EPI_BIAS_RESID) EVO_REQUIRE(p->bias != nullptr, "evo_gemm_smallm: bias epilogue without bias");
-  if (p->epilogue == EVO_EPI_RESID || p->epilogue == EVO_EPI_BIAS_RESID) EVO_REQUIRE(p->residual != nullptr, "evo_gemm_smallm: residual epilogue without residual");
+  if (check_smallm("evo_gemm_smallm", p)) return -1;
   if (p->M == 0) return 0;
-  switch (p->epilogue) {
-    case EVO_EPI_NONE: return launch_mb<EVO_EPI_NONE>(p, (cudaStream_t)stream);
-    case EVO_EPI_BIAS: return launch_mb<EVO_EPI_BIAS>(p, (cudaStream_t)stream);
-    case EVO_EPI_BIAS_RESID: return launch_mb<EVO_EPI_BIAS_RESID>(p, (cudaStream_t)stream);
-    case EVO_EPI_RESID: return launch_mb<EVO_EPI_RESID>(p, (cudaStream_t)stream);
-    case EVO_EPI_GELU_GATE: return launch_mb<EVO_EPI_GELU_GATE>(p, (cudaStream_t)stream);
+  return dispatch<false>("evo_gemm_smallm", p, nullptr, (cudaStream_t)stream);
+}
+
+extern "C" int evo_gemm_smallm_fp8(const evo_gemm_smallm_fp8_params* p, void* stream) {
+  if (check_smallm("evo_gemm_smallm_fp8", &p->base)) return -1;
+  EVO_REQUIRE(p->W_exp != nullptr, "evo_gemm_smallm_fp8: W_exp is required");
+  if (p->base.M == 0) return 0;
+  return dispatch<true>("evo_gemm_smallm_fp8", &p->base, p->W_exp, (cudaStream_t)stream);
+}
+
+extern "C" size_t evo_fp8_weight_bytes(int64_t N, int64_t K, int epilogue) {
+  const int R = epilogue == EVO_EPI_GELU_GATE ? 2 : 1;
+  if (N <= 0 || K <= 0 || K % BK != 0 || N % (R * WROWS) != 0) {
+    set_error("evo_fp8_weight_bytes: needs K a positive multiple of %d and N a positive multiple of %d (N %lld, K %lld)", BK, R * WROWS,
+              (long long)N, (long long)K);
+    return 0;
   }
-  set_error("evo_gemm_smallm: unknown epilogue %d", p->epilogue);
-  return -1;
+  return (size_t)N * (size_t)K;
+}
+
+extern "C" int evo_fp8_quantize_rows(void* W, int64_t N, int64_t K, int epilogue, void* W_q, void* W_exp, int* status, void* stream) {
+  EVO_REQUIRE(evo_fp8_weight_bytes(N, K, epilogue) != 0, "evo_fp8_quantize_rows: needs K a positive multiple of %d and N a positive multiple of %d "
+              "(N %lld, K %lld)", BK, epilogue == EVO_EPI_GELU_GATE ? 2 * WROWS : WROWS, (long long)N, (long long)K);
+  EVO_REQUIRE(N <= (1LL << 31) - 1, "evo_fp8_quantize_rows: N (%lld) too large", (long long)N);
+  EVO_REQUIRE(W != nullptr && W_q != nullptr && W_exp != nullptr && status != nullptr, "evo_fp8_quantize_rows: W, W_q, W_exp and status are required");
+  EVO_REQUIRE(((uintptr_t)W % 16) == 0 && ((uintptr_t)W_q % 16) == 0, "evo_fp8_quantize_rows: W and W_q must be 16-byte aligned");
+  const cudaStream_t st = (cudaStream_t)stream;
+  const int R = epilogue == EVO_EPI_GELU_GATE ? 2 : 1;
+  EVO_CUDA(cudaMemsetAsync(status, 0, sizeof(int), st));
+  fp8_row_exp_kernel<<<(unsigned)N, 256, 0, st>>>((const bf16*)W, (int)K, (int8_t*)W_exp, status);
+  if (int rc = check_launch("evo_fp8_quantize_rows")) return rc;
+  const long long n_chunks = N * K / 16;
+  const int grid = (int)std::min<long long>((n_chunks + 255) / 256, 64LL * std::max(1, device_sm_count()));
+  fp8_quantize_kernel<<<grid, 256, 0, st>>>((bf16*)W, K, (int)(K / BK), R, (const int8_t*)W_exp, (uint8_t*)W_q, status, n_chunks);
+  return check_launch("evo_fp8_quantize_rows");
 }

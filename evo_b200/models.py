@@ -53,14 +53,27 @@ def _resolve_config(model_name: str, config_path: Optional[str]) -> dict:
 
 
 def load_checkpoint(model_name: str = "evo-1-8k-base", config_path: Optional[str] = None, device: str = None,
-                    model_dir: Optional[str] = None, random_init: bool = False, seed: int = 0, streaming: bool = True, *args, **kwargs):
+                    model_dir: Optional[str] = None, random_init: bool = False, seed: int = 0, streaming: bool = True, *args,
+                    weights: str = "bf16", **kwargs):
     """HF snapshot -> safetensors -> StripedHyena on `device`.
 
     model_dir: use an already-downloaded snapshot directory instead of huggingface_hub.
     random_init: skip the checkpoint (benchmarks / tests on boxes without network) and keep the
     constructor's random initialisation, seeded.
     streaming: True (default) = tensor-by-tensor ingest straight into the device layouts; False = the reference's
-    host-state-dict sequence (kept as the comparator for the ingest tests)."""
+    host-state-dict sequence (kept as the comparator for the ingest tests).
+    weights: "bf16" (default) or "fp8": the model's linear-layer weights rounded onto an E4M3 grid with a power-of-two scale per
+    row, on the device after loading (StripedHyena.quantize_fp8): generation then streams one byte per weight."""
+    if weights not in WEIGHTS:
+        raise ValueError(f"weights={weights!r}: should be one of {', '.join(WEIGHTS)}")
+    model = _load(model_name, config_path, device, model_dir, random_init, seed, streaming)
+    return model.quantize_fp8() if weights == "fp8" else model
+
+
+WEIGHTS = ("bf16", "fp8")
+
+
+def _load(model_name, config_path, device, model_dir, random_init, seed, streaming):
     cfg = dotdict(_resolve_config(model_name, config_path))
 
     if random_init:
@@ -98,7 +111,8 @@ def load_checkpoint(model_name: str = "evo-1-8k-base", config_path: Optional[str
 
 
 class Evo:
-    """Evo('evo-1-8k-base') -> .model (StripedHyena protocol), .tokenizer."""
+    """Evo('evo-1-8k-base') -> .model (StripedHyena protocol), .tokenizer.  Evo(name, weights="fp8"): an FP8-weight model
+    (see load_checkpoint)."""
 
     def __init__(self, model_name: str = "evo-1-8k-base", device: str = None, **load_kwargs):
         if model_name not in MODEL_NAMES:

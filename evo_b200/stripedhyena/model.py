@@ -154,6 +154,40 @@ def pack_w12(l1: torch.Tensor, l2: torch.Tensor, ipad: int) -> torch.Tensor:
     return out.view(2 * ipad, k)
 
 
+def fp8_round_rows(w: torch.Tensor):
+    """Host reference of the FP8 weight rounding (evo_fp8_quantize_rows): an (N, K) bf16 matrix -> (W', q, e) with
+    W'[n, k] = q[n, k] 2^e[n], q torch.float8_e4m3fn (round to nearest even), e[n] = ceil(log2(amax_n / 448)) but at least -124
+    (so that W' is exactly a bf16 number), e = 0 for an all-zero row.  amax = m 2^p, m in [0.5, 1), 448 = 0.875 2^9."""
+    a = w.float().abs().amax(dim=1)
+    m, p = torch.frexp(a)
+    e = torch.where(m <= 0.875, p - 9, p - 8).clamp_min(-124)
+    e = torch.where(a > 0, e, torch.zeros_like(e))
+    q = torch.ldexp(w.float(), -e[:, None].float()).to(torch.float8_e4m3fn)
+    return torch.ldexp(q.float(), e[:, None].float()).to(torch.bfloat16), q, e.to(torch.int8)
+
+
+def _fp8_view(N: int, K: int, R: int):
+    """Axes of an (N, K) matrix as the FP8 decode layout sees them (csrc/gemm_smallm.cu): rows (tile, r, warpgroup, warp,
+    fragment row half, lane / 4), columns (k-block, 32-wide half, k16 step, fragment k half, lane % 4, pair element)."""
+    return (N // (128 * R), R, 2, 4, 2, 8, K // 64, 2, 2, 2, 4, 2)
+
+
+_FP8_ORDER = (0, 6, 1, 2, 3, 7, 5, 10, 8, 9, 4, 11)   # -> (tile, k-block, r, warpgroup, warp, half, lane, step, register, pair)
+
+
+def fp8_layout(q: torch.Tensor, gate: bool = False) -> torch.Tensor:
+    """(N, K) E4M3 weights -> the flat byte order evo_gemm_smallm_fp8 streams (gate: a packed w12, two 128-row groups per tile)."""
+    N, K = q.shape
+    return q.view(torch.uint8).reshape(_fp8_view(N, K, 2 if gate else 1)).permute(_FP8_ORDER).reshape(-1)
+
+
+def fp8_unlayout(flat: torch.Tensor, N: int, K: int, gate: bool = False) -> torch.Tensor:
+    """Inverse of fp8_layout: the flat bytes back to an (N, K) torch.float8_e4m3fn matrix."""
+    view = _fp8_view(N, K, 2 if gate else 1)
+    inv = sorted(range(len(_FP8_ORDER)), key=_FP8_ORDER.__getitem__)
+    return flat.view(torch.uint8).reshape([view[i] for i in _FP8_ORDER]).permute(inv).reshape(N, K).view(torch.float8_e4m3fn)
+
+
 def unpack_w12(w12: torch.Tensor, inner: int):
     ipad, k = w12.shape[0] // 2, w12.shape[1]
     v = w12.view(ipad // 128, 2, 128, k)
@@ -311,6 +345,12 @@ class StripedHyena(nn.Module):
         # programmatic dependent launch inside a decode step (evo_set_pdl): 0 off, 1 every kernel, 2 weight-streaming GEMMs only
         self.decode_pdl = int(os.environ.get("EVO_B200_DECODE_PDL", "4"))
         self._smallm_ws = None
+        # FP8 weights (quantize_fp8): the linear layers' parameters hold W' = q 2^e and the decode-step GEMMs stream (q, e), a
+        # cache built from W' like _packed.  _fp8_decode_bf16 runs those GEMMs on W' with the bf16 kernel instead (the tests'
+        # comparator: the two are bit-identical)
+        self._fp8_mode = False
+        self._fp8_decode_bf16 = False
+        self._fp8 = None
         self._tiled = None   # tile-major weight copies for the weight-streaming decode GEMMs
         self._decode = None  # cached CUDA graph of one decode step (see _decode_forward)
         self._loop = None    # cached CUDA graph of one step of the on-device generation loop (see decode_loop)
@@ -335,6 +375,8 @@ class StripedHyena(nn.Module):
     def load_state_dict(self, state_dict, strict: bool = True, **kw):
         out = super().load_state_dict(state_dict, strict=strict, **kw)
         self._invalidate()
+        if self._fp8_mode:
+            self._round_fp8()       # an FP8 model stays one: loaded weights are rounded onto the grid at once
         return out
 
     def _apply(self, fn, *a, **kw):
@@ -344,7 +386,76 @@ class StripedHyena(nn.Module):
 
     def _invalidate(self):
         """Drop everything built from the parameters or buffers (rotary tables from inv_freq) and the steps that captured it."""
-        self._packed = self._rope = self._tiled = self._decode = self._loop = None
+        self._packed = self._rope = self._tiled = self._decode = self._loop = self._fp8 = None
+
+    # ---- FP8 weights ----------------------------------------------------------------------------
+    def _fp8_weights(self):
+        """(block, name, parameter, gate layout) of every linear layer whose weight is held on the FP8 grid."""
+        for i, blk in enumerate(self.blocks):
+            if i in self._attn_idxs:
+                yield i, "in", blk.inner_mha_cls.Wqkv.weight, False
+                yield i, "out", blk.inner_mha_cls.out_proj.weight, False
+            else:
+                yield i, "in", blk.projections.weight, False
+                yield i, "out", blk.out_filter_dense.weight, False
+            yield i, "w12", blk.mlp.w12, True
+            yield i, "w3", blk.mlp.w3, False
+
+    def _quantize_rows(self, w, gate):
+        """evo_fp8_quantize_rows on one parameter: rounds it in place to W' and returns (q in the decode layout, e)."""
+        lib = _lib.lib()
+        N, K = w.shape
+        epi = EPI_GELU_GATE if gate else EPI_NONE
+        nbytes = lib.evo_fp8_weight_bytes(N, K, epi)
+        if nbytes == 0:
+            raise _lib.EvoError(lib.evo_last_error().decode())
+        q = torch.empty(nbytes, dtype=torch.uint8, device=w.device)
+        e = torch.empty(N, dtype=torch.int8, device=w.device)
+        status = torch.zeros(1, dtype=torch.int32, device=w.device)
+        check(lib.evo_fp8_quantize_rows(ptr(w), N, K, epi, ptr(q), ptr(e), ptr(status), self._stream()), "evo_fp8_quantize_rows")
+        if int(status.item()) != 0:
+            raise _lib.EvoError("evo_fp8_quantize_rows: a weight is not finite; the matrix was left unchanged")
+        return q, e
+
+    def _round_fp8(self):
+        with torch.no_grad():
+            ws = list(self._fp8_weights())
+            for _, _, w, _ in ws:
+                if w.device.type != "cuda" or w.dtype != torch.bfloat16:
+                    raise _lib.EvoError("quantize_fp8 runs on CUDA (sm_90a) with bf16 weights: move the model with .to('cuda:N') and call "
+                                        "to_bfloat16_except_poles_residues() first")
+            # refuse before anything is rounded, so that a refused model keeps every parameter
+            for i, name, w, _ in ws:
+                if not bool(torch.isfinite(w).all()):
+                    raise _lib.EvoError(f"quantize_fp8: block {i} {name} has a weight that is not finite; the model is unchanged")
+            with torch.cuda.device(ws[0][2].device):
+                for _, _, w, gate in ws:
+                    self._quantize_rows(w.data, gate)
+        self._invalidate()
+
+    def quantize_fp8(self):
+        """Make this an FP8 model: round the weight of every linear layer of every block (Wqkv / projections, out_proj /
+        out_filter_dense, the packed w12 and w3) onto an E4M3 grid with one power-of-two scale per output row, in place (see
+        fp8_round_rows).  Every path runs unchanged on the rounded bf16 weights W'; the decode-step GEMMs (batch <= 64) stream
+        the one-byte E4M3 copies instead, bit-identical to the bf16 kernel on W'.  The embedding stays bf16.  Idempotent;
+        state_dict() exports W' (an ordinary bf16 checkpoint), and load_state_dict() into an FP8 model rounds what it loads."""
+        self._round_fp8()
+        self._fp8_mode = True
+        return self
+
+    def _fp8_active(self):
+        return self._fp8_mode and not self._fp8_decode_bf16
+
+    def _ensure_fp8(self):
+        """The decode copies {block: {name: (q, e)}} of W' (quantizing W' again leaves it unchanged)."""
+        if self._fp8 is None:
+            cache = {}
+            with torch.no_grad(), torch.cuda.device(self.embedding_layer.weight.device):
+                for i, name, w, gate in self._fp8_weights():
+                    cache.setdefault(i, {})[name] = self._quantize_rows(w.data, gate)
+            cache["ptrs"] = tuple(t.data_ptr() for i in range(len(self.blocks)) for q in cache[i].values() for t in q)
+            self._fp8 = cache
+        return self._fp8
 
     # ---- weight packing (once per load / move) ---------------------------------------------
     def _ensure_packed(self):
@@ -408,8 +519,9 @@ class StripedHyena(nn.Module):
             p.c_peers, p.n_c_peers, p.peer_period, p.peer_inner, p.peer_row0 = C.cast(arr, C.c_void_p), n, period, inner, row0
         self._record(f"gemm/{N}x{K}/e{epi}/v{variant}", 2.0 * M * N * K, lambda: check(_lib.lib().evo_gemm(C.byref(p), self._stream()), "evo_gemm"))
 
-    def _gemm_smallm(self, a, w, out, M, N, K, epi, bias=None, resid=None):
-        """Decode-step linear layer (M <= 64): stream-K weight-streaming kernel, gate epilogue fused."""
+    def _gemm_smallm(self, a, w, out, M, N, K, epi, bias=None, resid=None, fp8=None):
+        """Decode-step linear layer (M <= 64): stream-K weight-streaming kernel, gate epilogue fused.  fp8 = (q, e) of W
+        (_ensure_fp8): the FP8-weight form streams those instead of w."""
         lib = _lib.lib()
         need = lib.evo_gemm_smallm_workspace(M, N, K, epi)
         ws = self._smallm_ws
@@ -422,6 +534,12 @@ class StripedHyena(nn.Module):
                              bias=bias.data_ptr() if bias is not None else None,
                              residual=resid.data_ptr() if resid is not None else None, ldr=n_out,
                              M=M, N=N, K=K, epilogue=epi, workspace=ws.data_ptr(), workspace_bytes=ws.numel())
+        if fp8 is not None:
+            p.W = fp8[0].data_ptr()
+            p8 = _lib.GemmSmallMFp8Params(base=p, W_exp=fp8[1].data_ptr())
+            self._record(f"gemm/{N}x{K}/e{epi}/streamk_fp8", 2.0 * M * N * K,
+                         lambda: check(lib.evo_gemm_smallm_fp8(C.byref(p8), self._stream()), "evo_gemm_smallm_fp8"))
+            return
         self._record(f"gemm/{N}x{K}/e{epi}/streamk", 2.0 * M * N * K, lambda: check(lib.evo_gemm_smallm(C.byref(p), self._stream()), "evo_gemm_smallm"))
 
     def _rmsnorm(self, x, scale, out, rows):
@@ -952,10 +1070,12 @@ class StripedHyena(nn.Module):
         wsel = (lambda i, name, w: tiled[i][name]) if tiled is not None else (lambda i, name, w: w)
         qkv_prep = lib.evo_decode_qkv_prep_rows if per_row else lib.evo_decode_qkv_prep
         decode_attn = lib.evo_decode_attn_rows if per_row else lib.evo_decode_attn
+        fp8 = self._ensure_fp8() if (streamk and self._fp8_active()) else None
+        f8 = (lambda i, name: fp8[i][name]) if fp8 is not None else (lambda i, name: None)
 
-        def lin(a, w, out, N, K, epi, bias=None, resid=None):
+        def lin(a, w, out, N, K, epi, bias=None, resid=None, q=None):
             if streamk:
-                self._gemm_smallm(a, w, out, B, N, K, epi, bias=bias, resid=resid)
+                self._gemm_smallm(a, w, out, B, N, K, epi, bias=bias, resid=resid, fp8=q)
             else:
                 self._gemm(a, w, out, B, N, K, epi, bias=bias, resid=resid, variant=G2)
 
@@ -969,7 +1089,7 @@ class StripedHyena(nn.Module):
             if i in self._attn_idxs:
                 mha = blk.inner_mha_cls
                 qkv = torch.empty(B, 3 * d, dtype=torch.bfloat16, device=dev)
-                lin(xn, wsel(i, "in", mha.Wqkv.weight), qkv, 3 * d, d, EPI_BIAS if mha.Wqkv.bias is not None else EPI_NONE, bias=mha.Wqkv.bias)
+                lin(xn, wsel(i, "in", mha.Wqkv.weight), qkv, 3 * d, d, EPI_BIAS if mha.Wqkv.bias is not None else EPI_NONE, bias=mha.Wqkv.bias, q=f8(i, "in"))
                 cache = mha_ip.key_value_memory_dict[i]
                 ctx = xn
                 if shared is not None:
@@ -982,26 +1102,26 @@ class StripedHyena(nn.Module):
                     check(decode_attn(ptr(qkv), ptr(cache), ptr(ctx), ptr(pos_dev), B, H, hd, cache.shape[1], nsplit,
                                               1.0 / math.sqrt(hd), ptr(ws), nws, self._stream()), "evo_decode_attn")
                 lin(ctx, wsel(i, "out", mha.out_proj.weight), u2, d, d, EPI_BIAS_RESID if mha.out_proj.bias is not None else EPI_RESID,
-                    bias=mha.out_proj.bias, resid=u)
+                    bias=mha.out_proj.bias, resid=u, q=f8(i, "out"))
             else:
                 z = torch.empty(B, 3 * d, dtype=torch.bfloat16, device=dev)
-                lin(xn, wsel(i, "in", blk.projections.weight), z, 3 * d, d, EPI_BIAS, bias=blk.projections.bias)
+                lin(xn, wsel(i, "in", blk.projections.weight), z, 3 * d, d, EPI_BIAS, bias=blk.projections.bias, q=f8(i, "in"))
                 y = xn
                 check(lib.evo_hyena_step(ptr(z), ptr(y), ptr(hy_ip.fir_state_dict[i]), ptr(torch.view_as_real(hy_ip.state_dict[i])),
                                          *map(C.c_void_p, blk.filter.ptrs().values()), B, d, cfg.state_size, H, self._stream()), "evo_hyena_step")
-                lin(y, wsel(i, "out", blk.out_filter_dense.weight), u2, d, d, EPI_BIAS_RESID, bias=blk.out_filter_dense.bias, resid=u)
+                lin(y, wsel(i, "out", blk.out_filter_dense.weight), u2, d, d, EPI_BIAS_RESID, bias=blk.out_filter_dense.bias, resid=u, q=f8(i, "out"))
             pk = self._packed[i]
             xn2 = xn
             self._rmsnorm(u2, blk.post_norm.scale, xn2, B)
             g = torch.empty(B, pk["ipad"], dtype=torch.bfloat16, device=dev)
             if streamk:
-                self._gemm_smallm(xn2, pk["w12"], g, B, 2 * pk["ipad"], d, EPI_GELU_GATE)
+                self._gemm_smallm(xn2, pk["w12"], g, B, 2 * pk["ipad"], d, EPI_GELU_GATE, fp8=f8(i, "w12"))
             else:
                 t = torch.empty(B, 2 * pk["ipad"], dtype=torch.bfloat16, device=dev)
                 self._gemm(xn2, wsel(i, "w12", pk["w12"]), t, B, 2 * pk["ipad"], d, EPI_NONE, variant=G2)
                 check(lib.evo_gelu_gate_interleaved(ptr(t), ptr(g), B, pk["ipad"], self._stream()), "evo_gelu_gate_interleaved")
             u = torch.empty_like(u2)
-            lin(g, wsel(i, "w3", pk["w3"]), u, d, pk["ipad"], EPI_RESID, resid=u2)
+            lin(g, wsel(i, "w3", pk["w3"]), u, d, pk["ipad"], EPI_RESID, resid=u2, q=f8(i, "w3"))
         u = self._final_norm(u)
         logits = torch.empty(B, V, dtype=torch.bfloat16, device=dev)
         lin(u, tiled["unembed"] if tiled is not None else self.unembed.weight, logits, V, d, EPI_NONE)
@@ -1289,8 +1409,10 @@ class StripedHyena(nn.Module):
             return picked[:, :n_out], kept[:, :n_out]
 
     def _graph_ptrs(self):
-        """Addresses a captured step bakes in besides the state tensors: rope tables and the stream-K workspace."""
-        return (tuple(t.data_ptr() for t in (self._rope or ())), self._smallm_ws.data_ptr() if self._smallm_ws is not None else 0)
+        """Addresses a captured step bakes in besides the state tensors: rope tables, the stream-K workspace and, for an FP8
+        model, its decode copies (none when _fp8_decode_bf16 selects the bf16 kernel)."""
+        return (tuple(t.data_ptr() for t in (self._rope or ())), self._smallm_ws.data_ptr() if self._smallm_ws is not None else 0,
+                self._fp8_active(), self._fp8["ptrs"] if self._fp8 is not None else ())
 
     def _step_key(self, ipd):
         """The state addresses a captured step bakes in, after making every Hyena state contiguous in place: each layer's

@@ -103,6 +103,24 @@ typedef struct {
 } evo_gemm_smallm_params;
 size_t evo_gemm_smallm_workspace(int64_t M, int64_t N, int64_t K, int epilogue);
 int evo_gemm_smallm(const evo_gemm_smallm_params* p, void* stream);
+/* FP8 weights for the decode step.  An FP8 model is a bf16 model whose linear-layer weights lie on an E4M3 grid with a
+ * power-of-two scale per output row: W'[n,k] = q[n,k] * 2^e[n], q E4M3 (OCP e4m3fn, round to nearest even),
+ * e[n] = ceil(log2(amax_n / 448)) but at least -124 (W' is then exactly a bf16 number), e = 0 and q = 0 for an all-zero row.
+ * evo_fp8_quantize_rows rounds an (N, K) bf16 W in place to W' and writes q in the layout evo_gemm_smallm_fp8 streams
+ * (private to the library: evo_fp8_weight_bytes() bytes, 16-byte aligned; the layout depends on whether the matrix is a
+ * GELU_GATE w12, given by `epilogue`) and the (N) int8 exponents W_exp.  A weight that is not finite refuses the whole matrix:
+ * *status (device int32) is set to 1 and W and W_q are left as they were (W_exp holds the exponents); 0 otherwise.
+ * Asynchronous on `stream`: read *status after it. */
+size_t evo_fp8_weight_bytes(int64_t N, int64_t K, int epilogue);
+int evo_fp8_quantize_rows(void* W, int64_t N, int64_t K, int epilogue, void* W_q, void* W_exp, int* status, void* stream);
+/* evo_gemm_smallm with base.W = the E4M3 weights of evo_fp8_quantize_rows and W_exp their row exponents: the same cut points,
+ * fix-up order, workspace and epilogues; the fp32 sum of column n is scaled by 2^e[n] before the epilogue.  Bit-identical to
+ * evo_gemm_smallm on W'. */
+typedef struct {
+  evo_gemm_smallm_params base;
+  const void* W_exp;             /* (N) int8 */
+} evo_gemm_smallm_fp8_params;
+int evo_gemm_smallm_fp8(const evo_gemm_smallm_fp8_params* p, void* stream);
 /* Programmatic dependent launch for the decode step.  0 = off (default); 1 = every decode-step kernel is launched with
  * programmatic stream serialization; 2 = only evo_gemm_smallm is (its weight prefetch then overlaps the small kernel or
  * the GEMM tail in front of it); 3 = evo_gemm_smallm and the few-row evo_rmsnorm; 4 = those and

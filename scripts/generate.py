@@ -16,7 +16,8 @@ header row (semantic_design's format) and generates them all in batches of up to
 --samples-per-prompt K repeats each CSV prompt K times, prompt-major (semantic_design's n_sample_per_prompt).
 --share-prompts sends the samples of one prompt (--prompt with --n-samples, or repeated CSV prompts) through shared-prompt
 sampling: each distinct prompt is prefilled once and its samples decode against one shared copy of its K,V.  The boolean
-flags keep the reference's `type=bool` parsing (any non-empty value is True).
+flags keep the reference's `type=bool` parsing (any non-empty value is True).  --fp8-weights generates with an FP8-weight
+model (Evo(weights="fp8")); scripts/score.py --fp8-weights scores under the same model.
 """
 import argparse
 
@@ -43,6 +44,8 @@ def build_parser():
     parser.add_argument('--seed', type=int, default=None, help='torch.manual_seed before sampling')
     parser.add_argument('--random-init', action='store_true', help='Skip the checkpoint download (random weights; smoke runs offline)')
     parser.add_argument('--model-dir', type=str, default=None, help='Directory of an already downloaded HF snapshot')
+    parser.add_argument('--fp8-weights', action='store_true',
+                        help='Round the linear-layer weights onto an FP8 (E4M3) grid, one power-of-two scale per row (Evo(weights="fp8"))')
     parser.add_argument('--prompts-csv', type=str, default=None,
                         help='CSV whose first column (after a header row) holds the prompts; generates every prompt once, batched whatever their lengths')
     parser.add_argument('--batch-size', type=int, default=64, help='Prompts per decode batch with --prompts-csv')
@@ -54,7 +57,8 @@ def build_parser():
 
 def main(argv=None):
     args = build_parser().parse_args(argv)
-    evo_model = Evo(args.model_name, device=args.device, random_init=args.random_init, model_dir=args.model_dir)
+    evo_model = Evo(args.model_name, device=args.device, random_init=args.random_init, model_dir=args.model_dir,
+                    weights='fp8' if args.fp8_weights else 'bf16')
     model, tokenizer = evo_model.model, evo_model.tokenizer
     model.eval()
     if args.seed is not None:

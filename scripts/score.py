@@ -10,7 +10,8 @@ Same arguments as the reference's scripts/score.py; what runs underneath is the 
 Biopython (evo_b200.frontend.read_fasta), sequences scored in LENGTH BUCKETS (--batch-size sequences or --max-tokens padded
 tokens per batch, whichever is hit first; the reference pads every file-order batch to its longest member), scores returned
 in file order.  --packed lays the sequences end to end without any padding instead (packs of --max-tokens tokens, one
-forward each).  --random-init / --model-dir are for boxes without network.
+forward each).  --random-init / --model-dir are for boxes without network.  --fp8-weights scores under the FP8-weight model
+(Evo(weights="fp8")), the model scripts/generate.py --fp8-weights samples from.
 """
 import argparse
 
@@ -31,12 +32,15 @@ def build_parser():
     parser.add_argument('--device', type=str, default='cuda:0', help='Device for scoring')
     parser.add_argument('--random-init', action='store_true', help='Skip the checkpoint download (random weights; smoke runs offline)')
     parser.add_argument('--model-dir', type=str, default=None, help='Directory of an already downloaded HF snapshot')
+    parser.add_argument('--fp8-weights', action='store_true',
+                        help='Round the linear-layer weights onto an FP8 (E4M3) grid, one power-of-two scale per row (Evo(weights="fp8"))')
     return parser
 
 
 def main(argv=None):
     args = build_parser().parse_args(argv)
-    evo_model = Evo(args.model_name, device=args.device, random_init=args.random_init, model_dir=args.model_dir)
+    evo_model = Evo(args.model_name, device=args.device, random_init=args.random_init, model_dir=args.model_dir,
+                    weights='fp8' if args.fp8_weights else 'bf16')
     model, tokenizer = evo_model.model, evo_model.tokenizer
     model.eval()
     _, seqs = read_fasta(args.input_fasta)

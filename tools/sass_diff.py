@@ -3,7 +3,8 @@
     python tools/sass_diff.py PARENT/evo_b200/build/hyena.o evo_b200/build/hyena.o
 
 Kernels are keyed by their demangled name without the argument list; a trailing `false` template flag (the RESUME form of
-hyena_scan_ms_kernel, the PREFIX form of attn_fwd_kernel) is dropped, so a pre-existing instantiation lines up with the one
+hyena_scan_ms_kernel, the PREFIX form of attn_fwd_kernel, the FP8
+form of gemm_smallm_kernel) is dropped, so a pre-existing instantiation lines up with the one
 it was before the flag existed.  Compare object files, not the linked library: linking moves global addresses.  Exit code 1
 if a pre-existing kernel's SASS changed or disappeared."""
 import re
@@ -34,6 +35,8 @@ def kernels(path):
         key = re.sub(r"<(true|false), (true|false), false>$", r"<\1, \2>", key)
         if "attn_fwd_kernel" in key:
             key = re.sub(r"<(true|false), false>$", r"<\1>", key)
+        if "gemm_smallm_kernel" in key:
+            key = re.sub(r", false>$", ">", key)
         res[key] = body[mangled]
     return res
 
