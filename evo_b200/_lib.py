@@ -121,6 +121,7 @@ SIGNATURES = {
     "evo_fp8_weight_bytes": (C.c_size_t, [C.c_int64, C.c_int64, C.c_int]),
     "evo_fp8_quantize_rows": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "evo_gemm_smallm_fp8": (C.c_int, [C.POINTER(GemmSmallMFp8Params), C.c_void_p]),
+    "evo_fp8_dequant_rows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int, C.c_void_p, C.c_void_p]),
     "evo_set_pdl": (C.c_int, [C.c_int]),
     "evo_hyena_fwd_workspace": (C.c_size_t, [C.POINTER(HyenaParams)]),
     "evo_hyena_fwd": (C.c_int, [C.POINTER(HyenaParams), C.c_void_p, C.c_size_t, C.c_void_p]),

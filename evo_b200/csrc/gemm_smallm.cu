@@ -499,6 +499,41 @@ __global__ void fp8_quantize_kernel(bf16* W, long long K, int KB, int R, const i
   }
 }
 
+// dequantizer of the FP8 decode weights: W' = q 2^e, row-major, from the layout fp8_quantize_kernel wrote, through that kernel's
+// conversion and scaling (so the bits are those it left in W).  One CTA per (tile, k-block) block of R * 8192 bytes: the block is
+// read whole with 16-byte loads into shared memory; then each thread gathers 8 consecutive columns of one row (the pair of bytes
+// at the same place in four consecutive 16-byte chunks: lanes 4j .. 4j + 3 of the fragment layout) and stores them as one
+// 16-byte segment, so a warp writes four whole 128-byte row pieces.
+constexpr int DQ_THREADS = 256;
+
+__global__ void __launch_bounds__(DQ_THREADS) fp8_dequant_kernel(const uint8_t* __restrict__ q, const int8_t* __restrict__ w_exp,
+                                                                 bf16* __restrict__ W, long long K, int KB, int R) {
+  __shared__ __align__(16) uint8_t blk[2 * FP8_BLOCK];
+  const long long b = blockIdx.x, tile = b / KB;
+  const int kb = (int)(b - tile * KB);
+  const uint4* src = reinterpret_cast<const uint4*>(q + b * (long long)(R * FP8_BLOCK));
+  for (int c = threadIdx.x; c < R * FP8_BLOCK / 16; c += DQ_THREADS) reinterpret_cast<uint4*>(blk)[c] = src[c];
+  __syncthreads();
+  for (int s = threadIdx.x; s < R * WROWS * (BK / 8); s += DQ_THREADS) {
+    // row nr of the tile = (r, warpgroup, warp, register % 2, lane / 4); columns 8 seg .. 8 seg + 7 = (k16 step, register / 2)
+    const int nr = s / (BK / 8), seg = s % (BK / 8);
+    const int r = nr / WROWS, rr = nr % WROWS;
+    const int cw = rr / 64, warp = (rr % 64) / 16, reg = 2 * (seg % 2) + (rr % 16) / 8, ks = seg / 2;
+    const int at = (r * 512 + cw * 256 + warp * 64 + (ks / 2) * 32 + (rr % 8) * 4) * 16 + (ks % 2) * 8 + reg * 2;
+    const long long n = tile * R * WROWS + nr;
+    const float sc = pow2f(w_exp[n]);
+    uint32_t out[4];
+#pragma unroll
+    for (int l = 0; l < 4; ++l) {                            // lane % 4 = l: columns 2l, 2l + 1 of the segment
+      const __nv_fp8x2_storage_t q2 = *reinterpret_cast<const __nv_fp8x2_storage_t*>(blk + at + l * 16);
+      const __half2_raw hr = __nv_cvt_fp8x2_to_halfraw2(q2, __NV_E4M3);
+      const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&hr));
+      out[l] = pack_bf16(f.x * sc, f.y * sc);
+    }
+    *reinterpret_cast<uint4*>(W + n * K + (long long)kb * BK + seg * 8) = make_uint4(out[0], out[1], out[2], out[3]);
+  }
+}
+
 }  // namespace
 
 extern "C" size_t evo_gemm_smallm_workspace(int64_t M, int64_t N, int64_t K, int epilogue) {
@@ -547,4 +582,18 @@ extern "C" int evo_fp8_quantize_rows(void* W, int64_t N, int64_t K, int epilogue
   const int grid = (int)std::min<long long>((n_chunks + 255) / 256, 64LL * std::max(1, device_sm_count()));
   fp8_quantize_kernel<<<grid, 256, 0, st>>>((bf16*)W, K, (int)(K / BK), R, (const int8_t*)W_exp, (uint8_t*)W_q, status, n_chunks);
   return check_launch("evo_fp8_quantize_rows");
+}
+
+extern "C" int evo_fp8_dequant_rows(const void* W_q, const void* W_exp, int64_t N, int64_t K, int epilogue, void* W_out, void* stream) {
+  EVO_REQUIRE(evo_fp8_weight_bytes(N, K, epilogue) != 0, "evo_fp8_dequant_rows: needs K a positive multiple of %d and N a positive multiple of %d "
+              "(N %lld, K %lld)", BK, epilogue == EVO_EPI_GELU_GATE ? 2 * WROWS : WROWS, (long long)N, (long long)K);
+  EVO_REQUIRE(N <= (1LL << 31) - 1 && N / WROWS * (K / BK) <= (1LL << 31) - 1, "evo_fp8_dequant_rows: N * K (%lld x %lld) too large",
+              (long long)N, (long long)K);
+  EVO_REQUIRE(W_q != nullptr && W_exp != nullptr && W_out != nullptr, "evo_fp8_dequant_rows: W_q, W_exp and W_out are required");
+  EVO_REQUIRE(((uintptr_t)W_q % 16) == 0 && ((uintptr_t)W_out % 16) == 0, "evo_fp8_dequant_rows: W_q and W_out must be 16-byte aligned");
+  const int R = epilogue == EVO_EPI_GELU_GATE ? 2 : 1;
+  const long long blocks = N / (R * WROWS) * (K / BK);
+  fp8_dequant_kernel<<<(unsigned)blocks, DQ_THREADS, 0, (cudaStream_t)stream>>>((const uint8_t*)W_q, (const int8_t*)W_exp, (bf16*)W_out, K,
+                                                                                 (int)(K / BK), R);
+  return check_launch("evo_fp8_dequant_rows");
 }

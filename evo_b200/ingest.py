@@ -10,7 +10,12 @@ everything to the GPU: ~3x the checkpoint in host memory and a single-threaded c
     w12 / w3 buffers, see stripedhyena.model._GatedMLP) are applied ON THE DEVICE, so no tensor exists twice;
   * strict-mode semantics are kept: missing / unexpected / mis-shaped keys raise RuntimeError like
     load_state_dict(strict=True) (evo/models.py:147).
-Peak host memory: the staging ring (2 x the largest tensor); peak device memory: the model plus one staged tensor."""
+Peak host memory: the staging ring (2 x the largest tensor); peak device memory: the model plus one staged tensor.
+
+compact=True (weights="fp8-compact"): the linear-layer weights are never resident in bf16.  Each one is rounded to FP8 and kept
+as (q, e) (StripedHyena.quantize_fp8(compact=True)) as soon as it is complete on the device, and its bf16 staging is freed; a
+packed w12 is held in bf16 only until both of its halves (l1, l2) have arrived.  Peak device memory: the compact model plus the
+matrices still being assembled and one staged tensor."""
 from __future__ import annotations
 
 import json
@@ -21,6 +26,7 @@ from typing import Dict, Iterator, List, Tuple
 
 import numpy as np
 import torch
+import torch.nn.functional as F
 
 _DTYPES = {"BF16": (torch.bfloat16, 2), "F16": (torch.float16, 2), "F32": (torch.float32, 4), "F64": (torch.float64, 8),
            "I64": (torch.int64, 8), "I32": (torch.int32, 4), "U8": (torch.uint8, 1), "I8": (torch.int8, 1), "BOOL": (torch.bool, 1)}
@@ -141,11 +147,62 @@ def _place(dst, kind: str, name: str, src: torch.Tensor, errors: List[str]) -> N
     v[full + (1 if inner % 128 else 0):].zero_()
 
 
-def load_streaming(model, model_dir: str, device) -> Dict[str, int]:
-    """Fill `model` (already on `device`, parameters uninitialised) from the safetensors files in model_dir.
+class _CompactSink:
+    """Linear-layer weights of a compact FP8 model (their parameters already empty): checkpoint key -> the weight's slot.  Each
+    matrix is rounded and kept as (q, e) once complete; w12 is assembled in a packed bf16 buffer until l1 and l2 are both in."""
+
+    def __init__(self, model):
+        self.model, self.slots, self.pending = model, {}, {}
+        names = {id(m): n for n, m in model.named_modules()}
+        d = model.config.hidden_size
+        for _, name, mod, attr, gate in model._fp8_slots():
+            p = names[id(mod)]
+            if attr == "w12":
+                self.slots[f"{p}.l1.weight"] = (mod, attr, gate, 0, (mod.inner, d))
+                self.slots[f"{p}.l2.weight"] = (mod, attr, gate, 1, (mod.inner, d))
+            elif attr == "w3":
+                self.slots[f"{p}.l3.weight"] = (mod, attr, gate, None, (d, mod.inner))
+            else:
+                self.slots[f"{p}.weight"] = (mod, attr, gate, None, (3 * d if name == "in" else d, d))
+
+    @torch.no_grad()
+    def place(self, key: str, src: torch.Tensor, errors: List[str]) -> None:
+        mod, attr, gate, half, shape = self.slots[key]
+        if tuple(src.shape) != shape:
+            errors.append(f"size mismatch for {key}: copying a param with shape {tuple(src.shape)} from checkpoint, the shape in current model is {shape}.")
+            return
+        src = src.to(torch.bfloat16)
+        if attr == "w3":
+            w = F.pad(src, (0, mod.ipad - mod.inner))
+        elif attr == "w12":
+            w = self.pending.get(id(mod))
+            if w is None:
+                w = self.pending[id(mod)] = (src.new_zeros(2 * mod.ipad, shape[1]), set())
+            _, got = w
+            v = w[0].view(mod.ipad // 128, 2, 128, shape[1])[:, half]
+            full = mod.inner // 128
+            v[:full].copy_(src[:full * 128].view(full, 128, shape[1]))
+            if mod.inner % 128:
+                v[full, :mod.inner % 128].copy_(src[full * 128:])
+            got.add(half)
+            if len(got) < 2:
+                return
+            w = self.pending.pop(id(mod))[0]
+        else:
+            w = src.contiguous()
+        with torch.cuda.device(w.device):
+            self.model._hold_compact(mod, attr, *self.model._quantize_rows(w, gate))
+
+
+def load_streaming(model, model_dir: str, device, compact: bool = False) -> Dict[str, int]:
+    """Fill `model` (already on `device`, parameters uninitialised) from the safetensors files in model_dir.  compact: the
+    model's linear-layer parameters are empty and their weights arrive as compact FP8 (see the module docstring).
     Returns {"tensors", "bytes"}; raises RuntimeError on any strict-mode violation."""
     device = torch.device(device)
     targets = _targets(model)
+    sink = _CompactSink(model) if compact else None
+    if sink is not None:
+        targets.update({k: (sink, "fp8") for k in sink.slots})
     seen, unexpected, errors = set(), [], []
     stage = _Staging(device)
     nbytes = 0
@@ -156,7 +213,10 @@ def load_streaming(model, model_dir: str, device) -> Dict[str, int]:
                 unexpected.append(key)
                 continue
             dst, kind = targets[key]
-            _place(dst, kind, key, stage.to_device(raw, dt, shape), errors)
+            if kind == "fp8":
+                sink.place(key, stage.to_device(raw, dt, shape), errors)
+            else:
+                _place(dst, kind, key, stage.to_device(raw, dt, shape), errors)
             seen.add(key)
             nbytes += len(raw)
     if "embedding_layer.weight" in seen or "unembed.weight" in seen:                         # tied embeddings: either name fills both

@@ -63,17 +63,22 @@ def load_checkpoint(model_name: str = "evo-1-8k-base", config_path: Optional[str
     streaming: True (default) = tensor-by-tensor ingest straight into the device layouts; False = the reference's
     host-state-dict sequence (kept as the comparator for the ingest tests).
     weights: "bf16" (default) or "fp8": the model's linear-layer weights rounded onto an E4M3 grid with a power-of-two scale per
-    row, on the device after loading (StripedHyena.quantize_fp8): generation then streams one byte per weight."""
+    row, on the device after loading (StripedHyena.quantize_fp8): generation then streams one byte per weight.
+    "fp8-compact": the same model holding only the one-byte weights and row exponents of those layers (quantize_fp8(compact=True)),
+    the same outputs on every path in about a third of the FP8 model's linear-weight memory.  The streaming ingest never holds
+    those layers in bf16 (each is compacted as soon as it is loaded); random_init and streaming=False build the bf16 model
+    first and compact it afterwards, so their peak device memory is the bf16 model's."""
     if weights not in WEIGHTS:
         raise ValueError(f"weights={weights!r}: should be one of {', '.join(WEIGHTS)}")
-    model = _load(model_name, config_path, device, model_dir, random_init, seed, streaming)
-    return model.quantize_fp8() if weights == "fp8" else model
+    compact = weights == "fp8-compact"
+    model = _load(model_name, config_path, device, model_dir, random_init, seed, streaming, compact)
+    return model.quantize_fp8(compact=compact) if weights != "bf16" else model
 
 
-WEIGHTS = ("bf16", "fp8")
+WEIGHTS = ("bf16", "fp8", "fp8-compact")
 
 
-def _load(model_name, config_path, device, model_dir, random_init, seed, streaming):
+def _load(model_name, config_path, device, model_dir, random_init, seed, streaming, compact=False):
     cfg = dotdict(_resolve_config(model_name, config_path))
 
     if random_init:
@@ -102,17 +107,24 @@ def _load(model_name, config_path, device, model_dir, random_init, seed, streami
     # each checkpoint tensor goes mmap -> pinned staging -> device and is cast / packed there (evo_b200/ingest.py)
     from .ingest import load_streaming
     dev = torch.device(device) if device is not None else torch.device("cpu")
+    compact = compact and dev.type == "cuda"        # elsewhere quantize_fp8 refuses the model after an ordinary load
     with torch.device("meta"):
         model = StripedHyena(cfg)
     model.to_bfloat16_except_poles_residues()
+    if compact:                                     # the linear weights arrive as (q, e): their parameters are never allocated
+        for _, _, mod, attr, _ in model._fp8_slots():
+            getattr(mod, attr).data = torch.empty(0, dtype=torch.bfloat16, device="meta")
     model = model.to_empty(device=dev)
-    model.ingest_stats = load_streaming(model, model_dir, dev)
+    model.ingest_stats = load_streaming(model, model_dir, dev, compact=compact)
+    if compact:
+        model._fp8_mode = model._fp8_compact = True
+        model._invalidate()
     return model
 
 
 class Evo:
-    """Evo('evo-1-8k-base') -> .model (StripedHyena protocol), .tokenizer.  Evo(name, weights="fp8"): an FP8-weight model
-    (see load_checkpoint)."""
+    """Evo('evo-1-8k-base') -> .model (StripedHyena protocol), .tokenizer.  Evo(name, weights="fp8"): an FP8-weight model;
+    weights="fp8-compact": the same model keeping only the one-byte weights (see load_checkpoint)."""
 
     def __init__(self, model_name: str = "evo-1-8k-base", device: str = None, **load_kwargs):
         if model_name not in MODEL_NAMES:

@@ -129,16 +129,16 @@ class PeerUlysses:
             check(lib.evo_peer_wait(ptr(self.buf[off: off + w * 4]), 0, w - 1, self.epoch, stream()), "evo_peer_wait(flags)")))
 
 
-def _peer_attention(model, lib, pu, xn, mha, u, B, Lr, H, hd, rank, world, stream):
+def _peer_attention(model, lib, pu, i, xn, mha, u, B, Lr, H, hd, rank, world, stream):
     """One sequence-parallel attention layer with the re-shard fused into the GEMM / attention epilogues (PeerUlysses).
-    xn (Lr, D) = pre-norm output; returns ctx (Lr, D), this rank's tokens x all heads, ready for out_proj."""
+    xn (Lr, D) = pre-norm output of block i; returns ctx (Lr, D), this rank's tokens x all heads, ready for out_proj."""
     d = H * hd
     k = pu.calls % 2
     pu.calls += 1
     pu.epoch += 1
     cos_p, sin_p = model._rope_at(rank * Lr, Lr, xn.device)
     # Wqkv: bias + rotary + scatter to the head-owning ranks, tile by tile while the GEMM runs
-    model._gemm(xn, mha.Wqkv.weight, None, Lr, 3 * d, d, EPI_BIAS_ROPE, bias=mha.Wqkv.bias, ldc=3 * pu.dl, rope=(cos_p, sin_p, Lr, 2 * d),
+    model._gemm(xn, model.linear_weight(i, "in"), None, Lr, 3 * d, d, EPI_BIAS_ROPE, bias=mha.Wqkv.bias, ldc=3 * pu.dl, rope=(cos_p, sin_p, Lr, 2 * d),
                 peers=(pu.full_ptrs[k], world, d, pu.dl, rank * Lr))
     pu.signal_and_wait(model, lib, "q", stream)
     full = pu.full(k)                                   # (L, 3, Hl, hd): my heads, the whole sequence
@@ -248,21 +248,21 @@ def sequence_parallel_forward(model, ids_local: torch.Tensor, rank: int, world: 
             model._rmsnorm(u, blk.pre_norm.scale, xn, M)
             if i in model._attn_idxs and pu is not None:
                 mha = blk.inner_mha_cls
-                ctx = _peer_attention(model, lib, pu, xn, mha, u, B, Lr, H, hd, rank, world, stream)
+                ctx = _peer_attention(model, lib, pu, i, xn, mha, u, B, Lr, H, hd, rank, world, stream)
                 since_sync = 0           # the flag rounds are global synchronisation points
-                u2 = model._out_proj(mha, ctx, u)
+                u2 = model._out_proj(i, mha, ctx, u)
             elif i in model._attn_idxs:
                 mha = blk.inner_mha_cls
                 qkv = torch.empty(M, 3 * d, dtype=torch.bfloat16, device=dev)
-                model._qkv_rope(xn, mha, qkv, B, Lr, model._rope_at(rank * Lr, Lr, dev))
+                model._qkv_rope(i, xn, mha, qkv, B, Lr, model._rope_at(rank * Lr, Lr, dev))
                 ctx = xn
                 _ulysses_attention(model, lib, qkv, ctx, B, Lr, H, hd, rank, world, group, stream)
                 since_sync = 0           # the all-to-all is a global synchronisation point
-                u2 = model._out_proj(mha, ctx, u)
+                u2 = model._out_proj(i, mha, ctx, u)
             else:
                 f = blk.filter
                 z = torch.empty(M, 3 * d, dtype=torch.bfloat16, device=dev)
-                model._gemm(xn, blk.projections.weight, z, M, 3 * d, d, EPI_BIAS, bias=blk.projections.bias)
+                model._gemm(xn, model.linear_weight(i, "in"), z, M, 3 * d, d, EPI_BIAS, bias=blk.projections.bias)
                 tail = z.view(B, Lr, 3 * d)[:, -2:].contiguous()
                 if pc is not None:
                     if since_sync == pc.NBUF:
@@ -310,7 +310,7 @@ def sequence_parallel_forward(model, ids_local: torch.Tensor, rank: int, world: 
                 hp.y, hp.state_in, hp.state_out, hp.state_only, hp.reuse_segment_states = y.data_ptr(), s_in.data_ptr(), None, 0, 1
                 model._record("hyena", 8.0 * B * Lr * d, lambda: check(lib.evo_hyena_fwd(C.byref(hp), ptr(ws), n, stream()), "evo_hyena_fwd"))
                 u2 = torch.empty_like(u)
-                model._gemm(y, blk.out_filter_dense.weight, u2, M, d, d, EPI_BIAS_RESID, bias=blk.out_filter_dense.bias, resid=u)
+                model._gemm(y, model.linear_weight(i, "out"), u2, M, d, d, EPI_BIAS_RESID, bias=blk.out_filter_dense.bias, resid=u)
             u = model._mlp_residual(i, blk, u2, M)
         logits = model._logits(model._final_norm(u))
     return logits.view(B, Lr, V)

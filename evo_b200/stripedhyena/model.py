@@ -13,6 +13,7 @@ never calls a torch op on activations.  torch supplies device memory and the str
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes as C
 import math
 import numbers
@@ -351,6 +352,10 @@ class StripedHyena(nn.Module):
         self._fp8_mode = False
         self._fp8_decode_bf16 = False
         self._fp8 = None
+        # compact FP8 weights (quantize_fp8(compact=True)): the linear layers' (q, e) are the weights, held as non-persistent
+        # buffers <attr>_q / <attr>_exp beside an empty parameter; linear_weight() rebuilds W' into _w_scratch before each GEMM
+        self._fp8_compact = False
+        self._w_scratch = None
         self._tiled = None   # tile-major weight copies for the weight-streaming decode GEMMs
         self._decode = None  # cached CUDA graph of one decode step (see _decode_forward)
         self._loop = None    # cached CUDA graph of one step of the on-device generation loop (see decode_loop)
@@ -373,11 +378,22 @@ class StripedHyena(nn.Module):
         }
 
     def load_state_dict(self, state_dict, strict: bool = True, **kw):
+        if self._fp8_compact:
+            return self._load_compact(state_dict, strict, **kw)
         out = super().load_state_dict(state_dict, strict=strict, **kw)
         self._invalidate()
         if self._fp8_mode:
             self._round_fp8()       # an FP8 model stays one: loaded weights are rounded onto the grid at once
         return out
+
+    def state_dict(self, *args, **kw):
+        """The reference's keys and layouts.  A compact FP8 model exports W' (the bits a non-compact FP8 model holds), rebuilt
+        on the model's device from (q, e): the call allocates the bf16 size of the linear weights, which the returned tensors
+        then hold."""
+        if not self._fp8_compact:
+            return super().state_dict(*args, **kw)
+        with self._materialized():
+            return super().state_dict(*args, **kw)
 
     def _apply(self, fn, *a, **kw):
         out = super()._apply(fn, *a, **kw)
@@ -386,20 +402,95 @@ class StripedHyena(nn.Module):
 
     def _invalidate(self):
         """Drop everything built from the parameters or buffers (rotary tables from inv_freq) and the steps that captured it."""
-        self._packed = self._rope = self._tiled = self._decode = self._loop = self._fp8 = None
+        self._packed = self._rope = self._tiled = self._decode = self._loop = self._fp8 = self._w_scratch = None
 
     # ---- FP8 weights ----------------------------------------------------------------------------
+    def _slot(self, i, name):
+        """(owning module, attribute, gate layout) of block i's linear layer `name`: "in" (Wqkv / projections), "out" (out_proj /
+        out_filter_dense), "w12" (the packed l1 / l2) or "w3"."""
+        blk = self.blocks[i]
+        if name in ("w12", "w3"):
+            return blk.mlp, name, name == "w12"
+        if i in self._attn_idxs:
+            return (blk.inner_mha_cls.Wqkv if name == "in" else blk.inner_mha_cls.out_proj), "weight", False
+        return (blk.projections if name == "in" else blk.out_filter_dense), "weight", False
+
+    def _fp8_slots(self):
+        """(block, name, owning module, attribute, gate layout) of every linear layer whose weight is held on the FP8 grid."""
+        for i in range(len(self.blocks)):
+            for name in ("in", "out", "w12", "w3"):
+                yield (i, name) + self._slot(i, name)
+
     def _fp8_weights(self):
         """(block, name, parameter, gate layout) of every linear layer whose weight is held on the FP8 grid."""
-        for i, blk in enumerate(self.blocks):
-            if i in self._attn_idxs:
-                yield i, "in", blk.inner_mha_cls.Wqkv.weight, False
-                yield i, "out", blk.inner_mha_cls.out_proj.weight, False
-            else:
-                yield i, "in", blk.projections.weight, False
-                yield i, "out", blk.out_filter_dense.weight, False
-            yield i, "w12", blk.mlp.w12, True
-            yield i, "w3", blk.mlp.w3, False
+        for i, name, mod, attr, gate in self._fp8_slots():
+            yield i, name, getattr(mod, attr), gate
+
+    @staticmethod
+    def _compact_qe(mod, attr):
+        """The (q, e) buffers a compact FP8 model holds for mod.<attr>."""
+        return getattr(mod, attr + "_q"), getattr(mod, attr + "_exp")
+
+    def _dequant(self, q, e, gate, out):
+        """evo_fp8_dequant_rows: W' = q 2^e into out (N, K) bf16 on the current stream."""
+        N, K = e.numel(), q.numel() // e.numel()
+        self._record(f"fp8_dequant/{N}x{K}", 0.0, lambda: check(_lib.lib().evo_fp8_dequant_rows(
+            ptr(q), ptr(e), N, K, EPI_GELU_GATE if gate else EPI_NONE, ptr(out), self._stream()), "evo_fp8_dequant_rows"))
+        return out
+
+    def linear_weight(self, i, name):
+        """W' of block i's linear layer `name` ("in", "out", "w12" or "w3"; see _slot) as the GEMMs read it: (N, K) bf16 row-major,
+        w12 in its packed order.  A bf16 or FP8 model returns the parameter.  A compact FP8 model rebuilds W' from (q, e) into
+        one scratch buffer on the current stream and returns that buffer: it holds this matrix until the next call, so the GEMM
+        that reads it must be the next kernel to touch it on the same stream."""
+        mod, attr, gate = self._slot(i, name)
+        if not self._fp8_compact:
+            return getattr(mod, attr)
+        q, e = self._compact_qe(mod, attr)
+        if self._w_scratch is None:
+            n = max(self._compact_qe(m, a)[0].numel() for _, _, m, a, _ in self._fp8_slots())
+            self._w_scratch = torch.empty(n, dtype=torch.bfloat16, device=q.device)
+        return self._dequant(q, e, gate, self._w_scratch[:q.numel()].view(e.numel(), -1))
+
+    def _hold_compact(self, mod, attr, q, e):
+        """Keep (q, e) as mod.<attr>'s weights and free its bf16 storage (the parameter stays, empty, under its key)."""
+        mod.register_buffer(attr + "_q", q, persistent=False)
+        mod.register_buffer(attr + "_exp", e, persistent=False)
+        getattr(mod, attr).data = torch.empty(0, dtype=torch.bfloat16, device=q.device)
+
+    @contextlib.contextmanager
+    def _materialized(self):
+        """A compact model whose linear parameters hold W' (new tensors, rebuilt from (q, e)) inside the block, empty again after."""
+        slots = list(self._fp8_slots())
+        if self.embedding_layer.weight.device.type != "cuda":
+            raise _lib.EvoError("a compact FP8 model rebuilds its weights on CUDA (sm_90a): move it with .to('cuda:N') first")
+        try:
+            with torch.no_grad(), torch.cuda.device(self.embedding_layer.weight.device):
+                for _, _, mod, attr, gate in slots:
+                    q, e = self._compact_qe(mod, attr)
+                    getattr(mod, attr).data = self._dequant(q, e, gate, torch.empty(e.numel(), q.numel() // e.numel(), dtype=torch.bfloat16,
+                                                                                    device=q.device))
+            yield
+        finally:
+            for _, _, mod, attr, _ in slots:
+                getattr(mod, attr).data = torch.empty(0, dtype=torch.bfloat16, device=self._compact_qe(mod, attr)[0].device)
+
+    def _load_compact(self, state_dict, strict, **kw):
+        """load_state_dict into a compact FP8 model: a non-finite linear weight is refused before anything changes; otherwise
+        the parameters hold W' for the load (a key the load does not fill keeps its value), and what is loaded is rounded and
+        kept as (q, e) again.  Peak: the bf16 size of the linear weights."""
+        names = {id(m): n for n, m in self.named_modules()}
+        for _, _, mod, attr, _ in self._fp8_slots():
+            p = names[id(mod)]
+            for k in ([f"{p}.l1.weight", f"{p}.l2.weight"] if attr == "w12" else [f"{p}.l3.weight"] if attr == "w3" else [f"{p}.weight"]):
+                v = state_dict.get(k)
+                if torch.is_tensor(v) and v.is_floating_point() and not bool(torch.isfinite(v).all()):
+                    raise _lib.EvoError(f"load_state_dict: {k} has a weight that is not finite; the model is unchanged")
+        with self._materialized():
+            out = super().load_state_dict(state_dict, strict=strict, **kw)
+            self._round_fp8(compact=True)
+        self._invalidate()
+        return out
 
     def _quantize_rows(self, w, gate):
         """evo_fp8_quantize_rows on one parameter: rounds it in place to W' and returns (q in the decode layout, e)."""
@@ -417,42 +508,55 @@ class StripedHyena(nn.Module):
             raise _lib.EvoError("evo_fp8_quantize_rows: a weight is not finite; the matrix was left unchanged")
         return q, e
 
-    def _round_fp8(self):
+    def _round_fp8(self, compact=False):
+        """Round every linear weight in place to W'; compact: then keep its (q, e) instead of W' (_hold_compact)."""
         with torch.no_grad():
-            ws = list(self._fp8_weights())
-            for _, _, w, _ in ws:
+            ws = list(self._fp8_slots())
+            for _, _, mod, attr, _ in ws:
+                w = getattr(mod, attr)
                 if w.device.type != "cuda" or w.dtype != torch.bfloat16:
                     raise _lib.EvoError("quantize_fp8 runs on CUDA (sm_90a) with bf16 weights: move the model with .to('cuda:N') and call "
                                         "to_bfloat16_except_poles_residues() first")
             # refuse before anything is rounded, so that a refused model keeps every parameter
-            for i, name, w, _ in ws:
-                if not bool(torch.isfinite(w).all()):
+            for i, name, mod, attr, _ in ws:
+                if not bool(torch.isfinite(getattr(mod, attr)).all()):
                     raise _lib.EvoError(f"quantize_fp8: block {i} {name} has a weight that is not finite; the model is unchanged")
-            with torch.cuda.device(ws[0][2].device):
-                for _, _, w, gate in ws:
-                    self._quantize_rows(w.data, gate)
+            with torch.cuda.device(getattr(ws[0][2], ws[0][3]).device):
+                for _, _, mod, attr, gate in ws:
+                    q, e = self._quantize_rows(getattr(mod, attr).data, gate)
+                    if compact:
+                        self._hold_compact(mod, attr, q, e)
         self._invalidate()
 
-    def quantize_fp8(self):
+    def quantize_fp8(self, compact: bool = False):
         """Make this an FP8 model: round the weight of every linear layer of every block (Wqkv / projections, out_proj /
         out_filter_dense, the packed w12 and w3) onto an E4M3 grid with one power-of-two scale per output row, in place (see
         fp8_round_rows).  Every path runs unchanged on the rounded bf16 weights W'; the decode-step GEMMs (batch <= 64) stream
         the one-byte E4M3 copies instead, bit-identical to the bf16 kernel on W'.  The embedding stays bf16.  Idempotent;
-        state_dict() exports W' (an ordinary bf16 checkpoint), and load_state_dict() into an FP8 model rounds what it loads."""
-        self._round_fp8()
-        self._fp8_mode = True
+        state_dict() exports W' (an ordinary bf16 checkpoint), and load_state_dict() into an FP8 model rounds what it loads.
+
+        compact=True: keep only the one-byte weights q and the row exponents e of those layers (about half the bf16 bytes, a
+        third of the non-compact FP8 model's) and free their bf16 storage.  Since W' = q 2^e exactly, every path that reads W'
+        gets it rebuilt bit for bit into one scratch buffer (linear_weight, sized for the largest matrix) just before its GEMM:
+        the outputs are the non-compact FP8 model's on every path.  A compact model stays compact (quantize_fp8 leaves it
+        unchanged, load_state_dict rounds what it loads)."""
+        if self._fp8_compact:
+            return self
+        self._round_fp8(compact=compact)
+        self._fp8_mode, self._fp8_compact = True, compact
         return self
 
     def _fp8_active(self):
         return self._fp8_mode and not self._fp8_decode_bf16
 
     def _ensure_fp8(self):
-        """The decode copies {block: {name: (q, e)}} of W' (quantizing W' again leaves it unchanged)."""
+        """The decode copies {block: {name: (q, e)}} of W' (quantizing W' again leaves it unchanged); a compact model's own."""
         if self._fp8 is None:
             cache = {}
             with torch.no_grad(), torch.cuda.device(self.embedding_layer.weight.device):
-                for i, name, w, gate in self._fp8_weights():
-                    cache.setdefault(i, {})[name] = self._quantize_rows(w.data, gate)
+                for i, name, mod, attr, gate in self._fp8_slots():
+                    cache.setdefault(i, {})[name] = (self._compact_qe(mod, attr) if self._fp8_compact
+                                                     else self._quantize_rows(getattr(mod, attr).data, gate))
             cache["ptrs"] = tuple(t.data_ptr() for i in range(len(self.blocks)) for q in cache[i].values() for t in q)
             self._fp8 = cache
         return self._fp8
@@ -470,10 +574,15 @@ class StripedHyena(nn.Module):
                 raise _lib.EvoError(f"parameter {name} is {p.dtype}; call to_bfloat16_except_poles_residues() (evo/models.py:148)")
             if p.device != dev:
                 raise _lib.EvoError(f"parameter {name} is on {p.device}, expected {dev}")
+        if self._fp8_compact:       # the linear parameters are empty: their (q, e) buffers are the weights
+            for i, name, mod, attr, _ in self._fp8_slots():
+                q, e = self._compact_qe(mod, attr)
+                if q.device != dev or e.device != dev or q.dtype != torch.uint8 or e.dtype != torch.int8:
+                    raise _lib.EvoError(f"block {i} {name}: FP8 weights {q.dtype} / {e.dtype} on {q.device}, expected uint8 / int8 on {dev}")
         packed = {}
         for i, blk in enumerate(self.blocks):
-            # the MLP parameters already live in the GEMM layouts (see _GatedMLP): nothing is copied here
-            packed[i] = {"w12": blk.mlp.w12.data, "w3": blk.mlp.w3.data, "ipad": blk.mlp.ipad}
+            # the MLP parameters already live in the GEMM layouts (see _GatedMLP): nothing is copied here; linear_weight reads them
+            packed[i] = {"ipad": blk.mlp.ipad}
         hd = self.config.hidden_size // self.config.num_attention_heads
         base = self.config.get("rotary_emb_base") or 10000
         # flash_attn keeps the checkpoint's inv_freq buffer when it is fp32 and recomputes it in fp32 otherwise
@@ -530,12 +639,11 @@ class StripedHyena(nn.Module):
             ws = self._smallm_ws = torch.zeros(max(need, lib.evo_gemm_smallm_workspace(M, 256, 64, EPI_GELU_GATE)),
                                                dtype=torch.uint8, device=a.device)
         n_out = N // 2 if epi == EPI_GELU_GATE else N
-        p = GemmSmallMParams(A=a.data_ptr(), lda=K, W=w.data_ptr(), C=out.data_ptr(), ldc=n_out,
+        p = GemmSmallMParams(A=a.data_ptr(), lda=K, W=(w if fp8 is None else fp8[0]).data_ptr(), C=out.data_ptr(), ldc=n_out,
                              bias=bias.data_ptr() if bias is not None else None,
                              residual=resid.data_ptr() if resid is not None else None, ldr=n_out,
                              M=M, N=N, K=K, epilogue=epi, workspace=ws.data_ptr(), workspace_bytes=ws.numel())
         if fp8 is not None:
-            p.W = fp8[0].data_ptr()
             p8 = _lib.GemmSmallMFp8Params(base=p, W_exp=fp8[1].data_ptr())
             self._record(f"gemm/{N}x{K}/e{epi}/streamk_fp8", 2.0 * M * N * K,
                          lambda: check(lib.evo_gemm_smallm_fp8(C.byref(p8), self._stream()), "evo_gemm_smallm_fp8"))
@@ -565,9 +673,9 @@ class StripedHyena(nn.Module):
         xn = torch.empty_like(u)
         self._rmsnorm(u, blk.post_norm.scale, xn, M)
         g = torch.empty(M, pk["ipad"], dtype=torch.bfloat16, device=u.device)
-        self._gemm(xn, pk["w12"], g, M, 2 * pk["ipad"], d, EPI_GELU_GATE, ldc=pk["ipad"])
+        self._gemm(xn, self.linear_weight(i, "w12"), g, M, 2 * pk["ipad"], d, EPI_GELU_GATE, ldc=pk["ipad"])
         out = xn  # reuse
-        self._gemm(g, pk["w3"], out, M, d, pk["ipad"], EPI_RESID, resid=u)
+        self._gemm(g, self.linear_weight(i, "w3"), out, M, d, pk["ipad"], EPI_RESID, resid=u)
         return out
 
     def _launch_ws(self, kind, work, what, size, fn, p, *args):
@@ -602,7 +710,7 @@ class StripedHyena(nn.Module):
         xn = torch.empty_like(u)
         self._rmsnorm(u, blk.pre_norm.scale, xn, M)
         z = torch.empty(M, 3 * d, dtype=torch.bfloat16, device=dev)
-        self._gemm(xn, blk.projections.weight, z, M, 3 * d, d, EPI_BIAS, bias=blk.projections.bias)
+        self._gemm(xn, self.linear_weight(i, "in"), z, M, 3 * d, d, EPI_BIAS, bias=blk.projections.bias)
         y = xn  # (M, D) buffer reuse
         lib = _lib.lib()
         have_state = ip is not None and i in ip.fir_state_dict
@@ -624,7 +732,7 @@ class StripedHyena(nn.Module):
             if ip is not None:
                 ip.state_dict[i], ip.fir_state_dict[i] = torch.view_as_complex(st_out), fs_out
         u2 = torch.empty_like(u)
-        self._gemm(y, blk.out_filter_dense.weight, u2, M, d, d, EPI_BIAS_RESID, bias=blk.out_filter_dense.bias, resid=u)
+        self._gemm(y, self.linear_weight(i, "out"), u2, M, d, d, EPI_BIAS_RESID, bias=blk.out_filter_dense.bias, resid=u)
         return self._mlp_residual(i, blk, u2, M)
 
     def _hyena_varlen(self, i, f, z, y, vl, ip):
@@ -668,23 +776,23 @@ class StripedHyena(nn.Module):
         hd = self.config.hidden_size // self.config.num_attention_heads
         return mha.Wqkv.bias is not None and hd == 128
 
-    def _qkv_rope(self, xn, mha, qkv, B, L, rope):
-        """qkv (B*L, 3D) = Wqkv xn (+ bias), rotary on q and k from rope = (cos, sin) addresses of each sequence's L rows."""
+    def _qkv_rope(self, i, xn, mha, qkv, B, L, rope):
+        """qkv (B*L, 3D) = Wqkv xn (+ bias) of block i, rotary on q and k from rope = (cos, sin) addresses of each sequence's L rows."""
         cfg, lib = self.config, _lib.lib()
         d, H = cfg.hidden_size, cfg.num_attention_heads
         M = B * L
         if self._rope_fused(mha):
-            self._gemm(xn, mha.Wqkv.weight, qkv, M, 3 * d, d, EPI_BIAS_ROPE, bias=mha.Wqkv.bias, rope=(*rope, L, 2 * d))
+            self._gemm(xn, self.linear_weight(i, "in"), qkv, M, 3 * d, d, EPI_BIAS_ROPE, bias=mha.Wqkv.bias, rope=(*rope, L, 2 * d))
         else:
-            self._gemm(xn, mha.Wqkv.weight, qkv, M, 3 * d, d, EPI_BIAS if mha.Wqkv.bias is not None else EPI_NONE, bias=mha.Wqkv.bias)
+            self._gemm(xn, self.linear_weight(i, "in"), qkv, M, 3 * d, d, EPI_BIAS if mha.Wqkv.bias is not None else EPI_NONE, bias=mha.Wqkv.bias)
             self._record("rotary", 8.0 * M * d, lambda: check(lib.evo_rotary_qk(ptr(qkv), C.c_void_p(rope[0]), C.c_void_p(rope[1]), B, L, H, d // H,
                                                                                 self._stream()), "evo_rotary_qk"))
 
-    def _out_proj(self, mha, ctx, u):
-        """u + out_proj(ctx) as a new (M, D) tensor."""
+    def _out_proj(self, i, mha, ctx, u):
+        """u + out_proj(ctx) of block i as a new (M, D) tensor."""
         d = self.config.hidden_size
         u2 = torch.empty_like(u)
-        self._gemm(ctx, mha.out_proj.weight, u2, u.shape[0], d, d, EPI_BIAS_RESID if mha.out_proj.bias is not None else EPI_RESID,
+        self._gemm(ctx, self.linear_weight(i, "out"), u2, u.shape[0], d, d, EPI_BIAS_RESID if mha.out_proj.bias is not None else EPI_RESID,
                    bias=mha.out_proj.bias, resid=u)
         return u2
 
@@ -711,7 +819,7 @@ class StripedHyena(nn.Module):
         off = int(ip.seqlen_offset) if ip is not None else 0
         # packed: the (T, 64) tables of each row's in-sequence position, read as one sequence of L = T rows
         rope = tuple(t.data_ptr() for t in varlen.rope) if varlen is not None else self._rope_at(off, L, dev)
-        self._qkv_rope(xn, mha, qkv, B, L, rope)
+        self._qkv_rope(i, xn, mha, qkv, B, L, rope)
         ctx = xn  # reuse
         if varlen is not None:
             self._attention_varlen(i, qkv, ctx, varlen, ip)
@@ -730,7 +838,7 @@ class StripedHyena(nn.Module):
                 ap.kv_tok_stride, ap.kv_batch_stride, ap.Lk = 2 * d, cache.shape[1] * 2 * d, off + L
             causal_flops = 4.0 * B * H * hd * (L * (off + (L + 1) / 2.0))   # QK^T + PV over the visible (query, key) pairs
             self._launch_ws("attn", causal_flops, "evo_attn_fwd", lib.evo_attn_fwd_workspace, lib.evo_attn_fwd_ws, ap, ATTN_VARIANT)
-        return self._mlp_residual(i, blk, self._out_proj(mha, ctx, u), M)
+        return self._mlp_residual(i, blk, self._out_proj(i, mha, ctx, u), M)
 
     def _attention_varlen(self, i, qkv, ctx, vl, ip):
         """Packed sequences: causal attention within each sequence (evo_attn_fwd_varlen) on the packed qkv rows; with `ip`,
@@ -1034,13 +1142,7 @@ class StripedHyena(nn.Module):
         t = {}
         with torch.no_grad():
             for i, blk in enumerate(self.blocks):
-                pk = self._packed[i]
-                e = {"w12": self._tile64(pk["w12"]), "w3": self._tile64(pk["w3"])}
-                if i in self._attn_idxs:
-                    e["in"], e["out"] = self._tile64(blk.inner_mha_cls.Wqkv.weight.data), self._tile64(blk.inner_mha_cls.out_proj.weight.data)
-                else:
-                    e["in"], e["out"] = self._tile64(blk.projections.weight.data), self._tile64(blk.out_filter_dense.weight.data)
-                t[i] = e
+                t[i] = {name: self._tile64(self.linear_weight(i, name).data) for name in ("in", "out", "w12", "w3")}
             t["unembed"] = self._tile64(self.unembed.weight.data)
         self._tiled = t
         return t
@@ -1065,19 +1167,36 @@ class StripedHyena(nn.Module):
         lib = _lib.lib()
         mha_ip, hy_ip = ipd["mha"], ipd["hyena"]
         streamk = self.decode_streamk and B <= 64
-        tiled = self._ensure_tiled() if (self.decode_tiled and not streamk) else None
+        # a compact FP8 model never builds the tile-major copies: they would hold W' again (variant 2 gives variant 3's bits)
+        tiled = self._ensure_tiled() if (self.decode_tiled and not streamk and not self._fp8_compact) else None
         G2 = 3 if tiled is not None else 2       # weight-streaming tiles (3: tile-major weights)
-        wsel = (lambda i, name, w: tiled[i][name]) if tiled is not None else (lambda i, name, w: w)
         qkv_prep = lib.evo_decode_qkv_prep_rows if per_row else lib.evo_decode_qkv_prep
         decode_attn = lib.evo_decode_attn_rows if per_row else lib.evo_decode_attn
         fp8 = self._ensure_fp8() if (streamk and self._fp8_active()) else None
-        f8 = (lambda i, name: fp8[i][name]) if fp8 is not None else (lambda i, name: None)
 
-        def lin(a, w, out, N, K, epi, bias=None, resid=None, q=None):
-            if streamk:
-                self._gemm_smallm(a, w, out, B, N, K, epi, bias=bias, resid=resid, fp8=q)
-            else:
+        def lin(a, w, out, N, K, epi, bias=None, resid=None):
+            """w: a weight, or (block, name) of a linear layer: its (q, e) when the FP8 kernel streams them, otherwise its tile-major
+            copy or W' (linear_weight: for a compact model, rebuilt just now into the scratch)."""
+            q, scratch = None, False
+            if isinstance(w, tuple):
+                if fp8 is not None:
+                    q, w = fp8[w[0]][w[1]], None
+                elif tiled is not None:
+                    w = tiled[w[0]][w[1]]
+                else:
+                    w, scratch = self.linear_weight(*w), self._fp8_compact
+            if not streamk:
                 self._gemm(a, w, out, B, N, K, epi, bias=bias, resid=resid, variant=G2)
+            elif scratch:
+                # the stream-K kernel fetches its first weight tiles before griddepcontrol.wait: under programmatic dependent
+                # launch it could read the scratch before the dequant in front of it has finished writing it
+                prev = lib.evo_set_pdl(0)
+                try:
+                    self._gemm_smallm(a, w, out, B, N, K, epi, bias=bias, resid=resid)
+                finally:
+                    lib.evo_set_pdl(prev)
+            else:
+                self._gemm_smallm(a, w, out, B, N, K, epi, bias=bias, resid=resid, fp8=q)
 
         u = self._embed(x)
         n_sm = torch.cuda.get_device_properties(dev).multi_processor_count
@@ -1089,7 +1208,7 @@ class StripedHyena(nn.Module):
             if i in self._attn_idxs:
                 mha = blk.inner_mha_cls
                 qkv = torch.empty(B, 3 * d, dtype=torch.bfloat16, device=dev)
-                lin(xn, wsel(i, "in", mha.Wqkv.weight), qkv, 3 * d, d, EPI_BIAS if mha.Wqkv.bias is not None else EPI_NONE, bias=mha.Wqkv.bias, q=f8(i, "in"))
+                lin(xn, (i, "in"), qkv, 3 * d, d, EPI_BIAS if mha.Wqkv.bias is not None else EPI_NONE, bias=mha.Wqkv.bias)
                 cache = mha_ip.key_value_memory_dict[i]
                 ctx = xn
                 if shared is not None:
@@ -1101,27 +1220,26 @@ class StripedHyena(nn.Module):
                     ws = torch.empty(nws, dtype=torch.uint8, device=dev)
                     check(decode_attn(ptr(qkv), ptr(cache), ptr(ctx), ptr(pos_dev), B, H, hd, cache.shape[1], nsplit,
                                               1.0 / math.sqrt(hd), ptr(ws), nws, self._stream()), "evo_decode_attn")
-                lin(ctx, wsel(i, "out", mha.out_proj.weight), u2, d, d, EPI_BIAS_RESID if mha.out_proj.bias is not None else EPI_RESID,
-                    bias=mha.out_proj.bias, resid=u, q=f8(i, "out"))
+                lin(ctx, (i, "out"), u2, d, d, EPI_BIAS_RESID if mha.out_proj.bias is not None else EPI_RESID, bias=mha.out_proj.bias, resid=u)
             else:
                 z = torch.empty(B, 3 * d, dtype=torch.bfloat16, device=dev)
-                lin(xn, wsel(i, "in", blk.projections.weight), z, 3 * d, d, EPI_BIAS, bias=blk.projections.bias, q=f8(i, "in"))
+                lin(xn, (i, "in"), z, 3 * d, d, EPI_BIAS, bias=blk.projections.bias)
                 y = xn
                 check(lib.evo_hyena_step(ptr(z), ptr(y), ptr(hy_ip.fir_state_dict[i]), ptr(torch.view_as_real(hy_ip.state_dict[i])),
                                          *map(C.c_void_p, blk.filter.ptrs().values()), B, d, cfg.state_size, H, self._stream()), "evo_hyena_step")
-                lin(y, wsel(i, "out", blk.out_filter_dense.weight), u2, d, d, EPI_BIAS_RESID, bias=blk.out_filter_dense.bias, resid=u, q=f8(i, "out"))
+                lin(y, (i, "out"), u2, d, d, EPI_BIAS_RESID, bias=blk.out_filter_dense.bias, resid=u)
             pk = self._packed[i]
             xn2 = xn
             self._rmsnorm(u2, blk.post_norm.scale, xn2, B)
             g = torch.empty(B, pk["ipad"], dtype=torch.bfloat16, device=dev)
             if streamk:
-                self._gemm_smallm(xn2, pk["w12"], g, B, 2 * pk["ipad"], d, EPI_GELU_GATE, fp8=f8(i, "w12"))
+                lin(xn2, (i, "w12"), g, 2 * pk["ipad"], d, EPI_GELU_GATE)
             else:
                 t = torch.empty(B, 2 * pk["ipad"], dtype=torch.bfloat16, device=dev)
-                self._gemm(xn2, wsel(i, "w12", pk["w12"]), t, B, 2 * pk["ipad"], d, EPI_NONE, variant=G2)
+                lin(xn2, (i, "w12"), t, 2 * pk["ipad"], d, EPI_NONE)
                 check(lib.evo_gelu_gate_interleaved(ptr(t), ptr(g), B, pk["ipad"], self._stream()), "evo_gelu_gate_interleaved")
             u = torch.empty_like(u2)
-            lin(g, wsel(i, "w3", pk["w3"]), u, d, pk["ipad"], EPI_RESID, resid=u2, q=f8(i, "w3"))
+            lin(g, (i, "w3"), u, d, pk["ipad"], EPI_RESID, resid=u2)
         u = self._final_norm(u)
         logits = torch.empty(B, V, dtype=torch.bfloat16, device=dev)
         lin(u, tiled["unembed"] if tiled is not None else self.unembed.weight, logits, V, d, EPI_NONE)
@@ -1410,9 +1528,12 @@ class StripedHyena(nn.Module):
 
     def _graph_ptrs(self):
         """Addresses a captured step bakes in besides the state tensors: rope tables, the stream-K workspace and, for an FP8
-        model, its decode copies (none when _fp8_decode_bf16 selects the bf16 kernel)."""
+        model, its decode copies (none when _fp8_decode_bf16 selects the bf16 kernel); for a compact one, its (q, e) and the
+        scratch W' is rebuilt into."""
+        fp8 = self._ensure_fp8() if self._fp8_compact else self._fp8
         return (tuple(t.data_ptr() for t in (self._rope or ())), self._smallm_ws.data_ptr() if self._smallm_ws is not None else 0,
-                self._fp8_active(), self._fp8["ptrs"] if self._fp8 is not None else ())
+                self._fp8_active(), fp8["ptrs"] if fp8 is not None else (),
+                self._w_scratch.data_ptr() if self._w_scratch is not None else 0)
 
     def _step_key(self, ipd):
         """The state addresses a captured step bakes in, after making every Hyena state contiguous in place: each layer's

@@ -113,6 +113,11 @@ int evo_gemm_smallm(const evo_gemm_smallm_params* p, void* stream);
  * Asynchronous on `stream`: read *status after it. */
 size_t evo_fp8_weight_bytes(int64_t N, int64_t K, int epilogue);
 int evo_fp8_quantize_rows(void* W, int64_t N, int64_t K, int epilogue, void* W_q, void* W_exp, int* status, void* stream);
+/* The inverse: W_out (N, K) row-major bf16 = W' = q * 2^e from the W_q and W_exp that evo_fp8_quantize_rows wrote, in the row
+ * order the quantized matrix had (a GELU_GATE w12: its interleaved order), bit for bit the W' that call left in W.  Same N, K and
+ * epilogue rules as evo_fp8_weight_bytes; W_q and W_out 16-byte aligned.  Reads N*K + N bytes, writes 2*N*K.  Asynchronous on
+ * `stream`; a compact FP8 model runs it into one scratch buffer before each GEMM that reads W'. */
+int evo_fp8_dequant_rows(const void* W_q, const void* W_exp, int64_t N, int64_t K, int epilogue, void* W_out, void* stream);
 /* evo_gemm_smallm with base.W = the E4M3 weights of evo_fp8_quantize_rows and W_exp their row exponents: the same cut points,
  * fix-up order, workspace and epilogues; the fp32 sum of column n is scaled by 2^e[n] before the epilogue.  Bit-identical to
  * evo_gemm_smallm on W'. */

@@ -17,7 +17,8 @@ header row (semantic_design's format) and generates them all in batches of up to
 --share-prompts sends the samples of one prompt (--prompt with --n-samples, or repeated CSV prompts) through shared-prompt
 sampling: each distinct prompt is prefilled once and its samples decode against one shared copy of its K,V.  The boolean
 flags keep the reference's `type=bool` parsing (any non-empty value is True).  --fp8-weights generates with an FP8-weight
-model (Evo(weights="fp8")); scripts/score.py --fp8-weights scores under the same model.
+model (Evo(weights="fp8")); scripts/score.py --fp8-weights scores under the same model.  --fp8-compact uses the same FP8
+model holding only its one-byte weights (Evo(weights="fp8-compact")): the same tokens in about half the bf16 weight memory.
 """
 import argparse
 
@@ -46,6 +47,9 @@ def build_parser():
     parser.add_argument('--model-dir', type=str, default=None, help='Directory of an already downloaded HF snapshot')
     parser.add_argument('--fp8-weights', action='store_true',
                         help='Round the linear-layer weights onto an FP8 (E4M3) grid, one power-of-two scale per row (Evo(weights="fp8"))')
+    parser.add_argument('--fp8-compact', action='store_true',
+                        help='The --fp8-weights model keeping only its one-byte weights: same outputs, less memory (Evo(weights="fp8-compact"); '
+                             'takes precedence over --fp8-weights)')
     parser.add_argument('--prompts-csv', type=str, default=None,
                         help='CSV whose first column (after a header row) holds the prompts; generates every prompt once, batched whatever their lengths')
     parser.add_argument('--batch-size', type=int, default=64, help='Prompts per decode batch with --prompts-csv')
@@ -55,10 +59,15 @@ def build_parser():
     return parser
 
 
+def weights_arg(args):
+    """The Evo(weights=...) value the FP8 flags select."""
+    return 'fp8-compact' if args.fp8_compact else 'fp8' if args.fp8_weights else 'bf16'
+
+
 def main(argv=None):
     args = build_parser().parse_args(argv)
     evo_model = Evo(args.model_name, device=args.device, random_init=args.random_init, model_dir=args.model_dir,
-                    weights='fp8' if args.fp8_weights else 'bf16')
+                    weights=weights_arg(args))
     model, tokenizer = evo_model.model, evo_model.tokenizer
     model.eval()
     if args.seed is not None:

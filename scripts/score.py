@@ -11,7 +11,8 @@ Biopython (evo_b200.frontend.read_fasta), sequences scored in LENGTH BUCKETS (--
 tokens per batch, whichever is hit first; the reference pads every file-order batch to its longest member), scores returned
 in file order.  --packed lays the sequences end to end without any padding instead (packs of --max-tokens tokens, one
 forward each).  --random-init / --model-dir are for boxes without network.  --fp8-weights scores under the FP8-weight model
-(Evo(weights="fp8")), the model scripts/generate.py --fp8-weights samples from.
+(Evo(weights="fp8")), the model scripts/generate.py --fp8-weights samples from; --fp8-compact scores under that model
+held as one-byte weights only (Evo(weights="fp8-compact")): the same scores in less device memory.
 """
 import argparse
 
@@ -34,13 +35,21 @@ def build_parser():
     parser.add_argument('--model-dir', type=str, default=None, help='Directory of an already downloaded HF snapshot')
     parser.add_argument('--fp8-weights', action='store_true',
                         help='Round the linear-layer weights onto an FP8 (E4M3) grid, one power-of-two scale per row (Evo(weights="fp8"))')
+    parser.add_argument('--fp8-compact', action='store_true',
+                        help='The --fp8-weights model keeping only its one-byte weights: same outputs, less memory (Evo(weights="fp8-compact"); '
+                             'takes precedence over --fp8-weights)')
     return parser
+
+
+def weights_arg(args):
+    """The Evo(weights=...) value the FP8 flags select."""
+    return 'fp8-compact' if args.fp8_compact else 'fp8' if args.fp8_weights else 'bf16'
 
 
 def main(argv=None):
     args = build_parser().parse_args(argv)
     evo_model = Evo(args.model_name, device=args.device, random_init=args.random_init, model_dir=args.model_dir,
-                    weights='fp8' if args.fp8_weights else 'bf16')
+                    weights=weights_arg(args))
     model, tokenizer = evo_model.model, evo_model.tokenizer
     model.eval()
     _, seqs = read_fasta(args.input_fasta)
