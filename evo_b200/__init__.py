@@ -8,7 +8,8 @@ from .scoring import score_sequences, positional_entropies, prepare_batch, logit
 from .tokenizer import CharLevelTokenizer
 from .variants import score_variants, saturation_variants, apply_mutations
 from .embeddings import embed_sequences
+from .constraints import Constraints
 
 __all__ = ["Evo", "load_checkpoint", "generate", "Generator", "score_sequences", "positional_entropies",
            "prepare_batch", "logits_to_logprobs", "CharLevelTokenizer", "score_variants", "saturation_variants", "apply_mutations",
-           "embed_sequences"]
+           "embed_sequences", "Constraints"]

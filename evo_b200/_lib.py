@@ -106,6 +106,12 @@ class LoopParams(C.Structure):
                 ("seed", C.c_uint64), ("step0", C.c_int64)]
 
 
+class ConstraintParams(C.Structure):
+    _fields_ = [("next", C.c_void_p), ("allow", C.c_void_p), ("stop", C.c_void_p), ("token_symbol", C.c_void_p),
+                ("n_states", C.c_int32), ("n_tokens", C.c_int32),
+                ("state", C.c_void_p), ("length", C.c_void_p), ("n_stopped", C.c_void_p), ("index0", C.c_int64)]
+
+
 # name -> (restype, argtypes); every symbol include/evo_b200.h declares
 SIGNATURES = {
     "evo_last_error": (C.c_char_p, []),
@@ -155,6 +161,8 @@ SIGNATURES = {
     "evo_sample": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, C.c_uint64, C.c_uint64, C.c_void_p]),
     "evo_sample_step": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "evo_advance_counters": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
+    "evo_sample_constrained": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, C.c_uint64, C.c_uint64, C.c_void_p, C.c_void_p]),
+    "evo_sample_step_constrained": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "evo_unembed_score_workspace": (C.c_size_t, [C.c_int64, C.c_int]),
     "evo_unembed_score": (C.c_int, [C.POINTER(ScoreParams), C.c_void_p]),
     "evo_tokenize_pad": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_void_p]),

@@ -40,8 +40,11 @@ __device__ __forceinline__ float philox_uniform(uint64_t seed, uint64_t step, ui
 
 struct SampleCfg { int top_k; float top_p; float temperature; unsigned long long seed; };
 
-// returns the chosen vocabulary index (valid in every thread)
-__device__ int sample_row(const bf16* __restrict__ logits, int V, const SampleCfg cfg, uint64_t step, uint32_t row) {
+// returns the chosen vocabulary index (valid in every thread).  MASK: only entries whose thread passes allowed = true may be
+// picked -- they take ranks [0, n_allowed) among themselves (non-NaN first, then NaN, as without a mask), every disallowed entry
+// ranks after them and weighs like a -inf logit.  With every entry allowed the ranks, weights and pick are the unmasked ones.
+template <bool MASK>
+__device__ int sample_row(const bf16* __restrict__ logits, int V, const SampleCfg cfg, uint64_t step, uint32_t row, bool allowed = true) {
   __shared__ float s_val[MAXV];        // logits by index, later: by rank
   __shared__ int s_idx[MAXV];          // index by rank
   __shared__ float s_scan[2][MAXV];
@@ -55,7 +58,20 @@ __device__ int sample_row(const bf16* __restrict__ logits, int V, const SampleCf
   // A NaN compares false with everything, so finite entries take ranks [0, nfinite) among themselves; each NaN ranks after
   // every finite entry and after the NaNs of lower index, which makes the ranks a permutation of [0, V).
   int rank = 0;
-  if (t < V) {
+  if constexpr (MASK) {
+    // category: 0 allowed non-NaN, 1 allowed NaN, 2 disallowed; ranked by category, then by value (category 0), then by index
+    __shared__ unsigned char s_cat[MAXV];
+    const int cat = !allowed ? 2 : (mine == mine ? 0 : 1);
+    s_cat[t] = (unsigned char)cat;
+    __syncthreads();
+    if (t < V) {
+      for (int j = 0; j < V; ++j) {
+        const int cj = s_cat[j];
+        const float o = s_val[j];
+        rank += (cj < cat) || (cj == cat && (cat == 0 ? (o > mine) || (o == mine && j < t) : j < t));
+      }
+    }
+  } else if (t < V) {
     if (mine == mine) {
       for (int j = 0; j < V; ++j) {
         const float o = s_val[j];
@@ -76,8 +92,8 @@ __device__ int sample_row(const bf16* __restrict__ logits, int V, const SampleCf
   }
   const int k = cfg.top_k > 0 ? min(cfg.top_k, V) : V;
   // by rank; the temperature division is a bf16 tensor op in the reference (kept / temperature on bf16 logits)
-  float scaled = mine;
-  if (cfg.temperature != 1.0f) scaled = rbf(mine / cfg.temperature);
+  float scaled = (MASK && !allowed) ? -INFINITY : mine;
+  if (cfg.temperature != 1.0f) scaled = rbf(scaled / cfg.temperature);
   if (t < V) { s_idx[rank] = t; s_scan[0][rank] = scaled; }
   __syncthreads();
   const bool kept = t < k;
@@ -140,7 +156,7 @@ __device__ int sample_row(const bf16* __restrict__ logits, int V, const SampleCf
 
 __global__ void __launch_bounds__(MAXV) sample_kernel(const bf16* __restrict__ logits, long long* __restrict__ out, int V, SampleCfg cfg, unsigned long long step) {
   const int row = blockIdx.x;
-  const int pick = sample_row(logits + (long long)row * V, V, cfg, step, row);
+  const int pick = sample_row<false>(logits + (long long)row * V, V, cfg, step, row);
   if (threadIdx.x == 0) out[row] = pick;
 }
 
@@ -157,7 +173,7 @@ __global__ void __launch_bounds__(MAXV) sample_step_kernel(const bf16* __restric
     tok = P.forced[(long long)row * P.forced_stride + i];
   } else {
     const SampleCfg cfg = {P.top_k, P.top_p, P.temperature, (unsigned long long)P.seed};
-    tok = sample_row(logits + (long long)row * V, V, cfg, (uint64_t)(P.step0 + i), row);
+    tok = sample_row<false>(logits + (long long)row * V, V, cfg, (uint64_t)(P.step0 + i), row);
     const long long k = i - P.n_forced;
     if (k < P.n_out) {
       if (threadIdx.x == 0 && P.picked) P.picked[(long long)row * P.picked_stride + k] = tok;
@@ -166,6 +182,69 @@ __global__ void __launch_bounds__(MAXV) sample_step_kernel(const bf16* __restric
     }
   }
   if (threadIdx.x == 0) x[row] = tok;
+}
+
+// constrained sampling: thread t's token may be picked when the row's automaton state allows its symbol
+__device__ __forceinline__ bool token_allowed(const evo_constraint_params& C, int state, int t, int V) {
+  if (t >= V || t >= C.n_tokens) return false;
+  const int sym = C.token_symbol[t];
+  return sym >= 0 && ((C.allow[state] >> sym) & 1);
+}
+
+// after a running row picked `tok` as its generated token number `index`: advance its state; a stop state ends the row
+__device__ __forceinline__ void constraint_advance(const evo_constraint_params& C, int row, int state, long long tok, long long index) {
+  const int sym = C.token_symbol[tok];
+  if (sym < 0) return;                           // only when the state allows nothing (a hand-built table): nothing to advance by
+  const int ns = C.next[(long long)state * 4 + sym];
+  C.state[row] = ns;
+  if (C.stop[ns]) {
+    C.length[row] = index + 1;
+    atomicAdd(C.n_stopped, 1);
+  }
+}
+
+__global__ void __launch_bounds__(MAXV) sample_constrained_kernel(const bf16* __restrict__ logits, long long* __restrict__ out, int V, SampleCfg cfg,
+                                                                  unsigned long long step, const evo_constraint_params* __restrict__ cp) {
+  const int row = blockIdx.x;
+  const evo_constraint_params C = *cp;
+  if (C.length[row] >= 0) return;                // stopped: neither sampled nor advanced
+  const int s = C.state[row];
+  const int pick = sample_row<true>(logits + (long long)row * V, V, cfg, step, row, token_allowed(C, s, threadIdx.x, V));
+  if (threadIdx.x == 0) {
+    out[row] = pick;
+    constraint_advance(C, row, s, pick, C.index0);
+  }
+}
+
+// sample_step_kernel under an automaton: forced steps as there (the automaton's initial state covers the whole prompt); a
+// sampled step masks the row's logits, records its pick like sample_step_kernel and advances the row.  A stopped row keeps
+// feeding its last token and records nothing.
+__global__ void __launch_bounds__(MAXV) sample_step_constrained_kernel(const bf16* __restrict__ logits, long long* __restrict__ x, int V,
+                                                                       const evo_loop_params* __restrict__ lp, const evo_constraint_params* __restrict__ cp,
+                                                                       const long long* __restrict__ step_dev) {
+  pdl_launch_dependents(); pdl_wait();
+  const int row = blockIdx.x;
+  const long long i = *step_dev;
+  const evo_loop_params P = *lp;
+  if (i < P.n_forced) {
+    if (threadIdx.x == 0) x[row] = P.forced[(long long)row * P.forced_stride + i];
+    return;
+  }
+  const evo_constraint_params C = *cp;
+  if (C.length[row] >= 0) return;
+  const int s = C.state[row];
+  const SampleCfg cfg = {P.top_k, P.top_p, P.temperature, (unsigned long long)P.seed};
+  const long long tok = sample_row<true>(logits + (long long)row * V, V, cfg, (uint64_t)(P.step0 + i), row, token_allowed(C, s, threadIdx.x, V));
+  const long long k = i - P.n_forced;
+  if (k < P.n_out) {
+    if (threadIdx.x == 0 && P.picked) P.picked[(long long)row * P.picked_stride + k] = tok;
+    if (P.kept_logits && threadIdx.x < V)
+      P.kept_logits[((long long)row * P.n_out + k) * V + threadIdx.x] = __bfloat162float(logits[(long long)row * V + threadIdx.x]);
+  }
+  if (threadIdx.x == 0) {
+    x[row] = tok;
+    constraint_advance(C, row, s, tok, C.index0 + k);
+  }
 }
 
 __global__ void advance2_kernel(long long* a, long long* b, long long delta) {
@@ -193,6 +272,29 @@ extern "C" int evo_sample_step(const void* logits, int64_t* x, int B, int V, con
   EVO_CUDA(launch_pdl(sample_step_kernel, dim3(B), dim3((V + 31) / 32 * 32), 0, (cudaStream_t)stream, (const bf16*)logits, (long long*)x, V,
                       loop_params_dev, (const long long*)step_dev));
   return check_launch("evo_sample_step");
+}
+
+extern "C" int evo_sample_constrained(const void* logits, int64_t* out, int B, int V, int top_k, float top_p, float temperature,
+                                      uint64_t seed, uint64_t step, const evo_constraint_params* constraint_params_dev, void* stream) {
+  EVO_REQUIRE(V > 0 && V <= MAXV, "evo_sample_constrained: vocabulary %d unsupported (<= %d)", V, MAXV);
+  EVO_REQUIRE(!(top_p > 1.0f), "evo_sample_constrained: top-p should be in (0, 1]");
+  EVO_REQUIRE(temperature > 0.f || top_k == 1, "evo_sample_constrained: temperature must be positive");
+  EVO_REQUIRE(constraint_params_dev != nullptr, "evo_sample_constrained: needs constraint params");
+  if (B == 0) return 0;
+  const SampleCfg cfg = {top_k, top_p, temperature, (unsigned long long)seed};
+  sample_constrained_kernel<<<B, (V + 31) / 32 * 32, 0, (cudaStream_t)stream>>>((const bf16*)logits, (long long*)out, V, cfg, (unsigned long long)step,
+                                                                                 constraint_params_dev);
+  return check_launch("evo_sample_constrained");
+}
+
+extern "C" int evo_sample_step_constrained(const void* logits, int64_t* x, int B, int V, const evo_loop_params* loop_params_dev,
+                                           const evo_constraint_params* constraint_params_dev, const int64_t* step_dev, void* stream) {
+  EVO_REQUIRE(V > 0 && V <= MAXV, "evo_sample_step_constrained: vocabulary %d unsupported (<= %d)", V, MAXV);
+  EVO_REQUIRE(constraint_params_dev != nullptr, "evo_sample_step_constrained: needs constraint params");
+  if (B == 0) return 0;
+  EVO_CUDA(launch_pdl(sample_step_constrained_kernel, dim3(B), dim3((V + 31) / 32 * 32), 0, (cudaStream_t)stream, (const bf16*)logits, (long long*)x, V,
+                      loop_params_dev, constraint_params_dev, (const long long*)step_dev));
+  return check_launch("evo_sample_step_constrained");
 }
 
 extern "C" int evo_advance_counters(int64_t* a, int64_t* b, int64_t delta, void* stream) {

@@ -114,15 +114,24 @@ class Generator:
             print(f"\n[generate] in: {input_string} | out: {shown} | {_gb(dev):.2f} GB allocated")
         return picked, kept_logits, state
 
-    def _pick_device(self, head: torch.Tensor) -> torch.Tensor:
-        """One call of the device sampler (evo_sample) on (B, V) bf16 logits."""
+    def _pick_device(self, head: torch.Tensor, constraints=None) -> torch.Tensor:
+        """One call of the device sampler (evo_sample) on (B, V) bf16 logits; under a constraints.RowConstraints, one call of
+        evo_sample_constrained, which also advances its rows."""
         import ctypes as C
         from . import _lib
         out = torch.empty(head.shape[0], dtype=torch.long, device=head.device)
         seed = int(torch.randint(0, 2 ** 62, (1,)).item())
         head = head.to(torch.bfloat16).contiguous()
-        _lib.check(_lib.lib().evo_sample(_lib.ptr(head), _lib.ptr(out), head.shape[0], head.shape[1], int(self.top_k), float(self.top_p), float(self.temperature),
-                                         seed, 0, C.c_void_p(torch.cuda.current_stream(head.device).cuda_stream)), "evo_sample")
+        stream = C.c_void_p(torch.cuda.current_stream(head.device).cuda_stream)
+        if constraints is None:
+            _lib.check(_lib.lib().evo_sample(_lib.ptr(head), _lib.ptr(out), head.shape[0], head.shape[1], int(self.top_k), float(self.top_p), float(self.temperature),
+                                             seed, 0, stream), "evo_sample")
+            return out
+        cp = constraints.params()
+        cp_dev = torch.frombuffer(bytearray(C.string_at(C.addressof(cp), C.sizeof(cp))), dtype=torch.uint8).to(head.device)
+        _lib.check(_lib.lib().evo_sample_constrained(_lib.ptr(head), _lib.ptr(out), head.shape[0], head.shape[1], int(self.top_k), float(self.top_p),
+                                                     float(self.temperature), seed, 0, _lib.ptr(cp_dev), stream), "evo_sample_constrained")
+        constraints.index0 += 1
         return out
 
     # -- public ---------------------------------------------------------------------------
@@ -203,31 +212,56 @@ def _ragged_ids(prompt_seqs, model, tokenizer, n_tokens, prepend_bos):
     return ids, p0.device
 
 
-def _decode_batch(model, engine, tokenizer, head, state, starts, n_tokens):
+def _initial_states(automaton, ids):
+    """Each prompt's automaton state (None without constraints); raises ValueError before anything is launched when a
+    prompt has no live continuation."""
+    if automaton is None:
+        return None
+    return [automaton.initial_state(t) for t in ids]
+
+
+def _decode_batch(model, engine, tokenizer, head, state, starts, n_tokens, automaton=None, init_states=None):
     """First pick from the prefill's head logits, then n_tokens - 1 steps of the on-device loop at per-row positions `starts`;
-    returns (texts, mean log-likelihood scores) of the batch's rows, scored with the reference's alignment (Q3)."""
+    returns (texts, mean log-likelihood scores) of the batch's rows, scored with the reference's alignment (Q3).
+    With an automaton (constraints.compile) every pick is masked by it, rows start in `init_states`, and each row's text and
+    score end at its stop motif; the loop is skipped, or ends early, once every row has stopped."""
+    from .constraints import RowConstraints
     dev = head.device
-    picked = torch.empty(head.shape[0], n_tokens, dtype=torch.long, device=dev)
-    kept_logits = torch.empty(head.shape[0], n_tokens, tokenizer.vocab_size, dtype=torch.float, device=dev)
-    token = engine._pick_device(head)
+    B = head.shape[0]
+    picked = torch.empty(B, n_tokens, dtype=torch.long, device=dev)
+    kept_logits = torch.empty(B, n_tokens, tokenizer.vocab_size, dtype=torch.float, device=dev)
+    rows = None if automaton is None else RowConstraints(automaton, init_states, dev)
+    token = engine._pick_device(head, rows)
     kept_logits[:, 0], picked[:, 0] = head, token
-    if n_tokens > 1:
-        got, got_logits = model.decode_loop(token, state, n_tokens - 1, starts, n_out=n_tokens - 1,
-                                            top_k=engine.top_k, top_p=engine.top_p, temperature=engine.temperature)
+    loop_args = dict(n_out=n_tokens - 1, top_k=engine.top_k, top_p=engine.top_p, temperature=engine.temperature)
+    if rows is None:
+        if n_tokens > 1:
+            got, got_logits = model.decode_loop(token, state, n_tokens - 1, starts, **loop_args)
+            picked[:, 1:], kept_logits[:, 1:] = got, got_logits
+        decoded = tokenizer.detokenize_batch(picked)
+        # logits_to_logprobs(trim_bos=True) pairs logits[i] with token[i+1]: the reference's alignment (Q3)
+        per_token = logits_to_logprobs(kept_logits, picked).float().cpu().numpy()
+        return decoded, [float(np.mean(row)) for row in per_token]
+    if n_tokens > 1 and not (automaton.has_stop and int(rows.n_stopped.item()) == B):
+        got, got_logits, _ = model.decode_loop(token, state, n_tokens - 1, starts, constraints=rows, **loop_args)
         picked[:, 1:], kept_logits[:, 1:] = got, got_logits
-    decoded = tokenizer.detokenize_batch(picked)
-    # logits_to_logprobs(trim_bos=True) pairs logits[i] with token[i+1]: the reference's alignment (Q3)
+    lengths = [n if n >= 0 else n_tokens for n in rows.length.tolist()]
+    # columns past a row's length were never written: zero their token ids so the gather stays in range; their pairs are dropped
+    keep = torch.arange(n_tokens, device=dev)[None, :] < torch.tensor(lengths, device=dev)[:, None]
+    picked = torch.where(keep, picked, 0)
     per_token = logits_to_logprobs(kept_logits, picked).float().cpu().numpy()
-    return decoded, [float(np.mean(row)) for row in per_token]
+    texts = [tokenizer.detokenize(row[:n]) for row, n in zip(picked.tolist(), lengths)]
+    return texts, [float(np.mean(row[:n - 1])) if n > 1 else float("nan") for row, n in zip(per_token, lengths)]
 
 
-def _generate_shared(prompt_seqs, model, tokenizer, engine, n_tokens, prepend_bos, batch_size, verbose):
+def _generate_shared(prompt_seqs, model, tokenizer, engine, n_tokens, prepend_bos, batch_size, verbose, automaton=None):
     """generate(ragged=True, share_prompts=True): identical prompts form one group; each distinct prompt is prefilled once
     (StripedHyena.prefill_prefixes, packed) and its rows decode against its K,V as one shared prefix
     (StripedHyena.shared_decode_state + decode_loop), in batches of <= batch_size rows (frontend.shared_batches).  Texts and
     scores come back in input order."""
     from .frontend import shared_batches
     ids, _ = _ragged_ids(prompt_seqs, model, tokenizer, n_tokens, prepend_bos)
+    init = _initial_states(automaton, ids)
     groups, plan = shared_batches(ids, n_tokens, batch_size)
     last_batch = {g: k for k, (parts, _, _) in enumerate(plan) for g, _ in parts}
     live = {}                                     # group -> (its prefill's prefixes, its index there), until its last batch
@@ -245,7 +279,8 @@ def _generate_shared(prompt_seqs, model, tokenizer, engine, n_tokens, prepend_bo
                 del live[g]
         rows = [r for _, rr in parts for r in rr]
         starts = torch.tensor([len(ids[r]) for r in rows], dtype=torch.int64)
-        decoded, got = _decode_batch(model, engine, tokenizer, head, state, starts, n_tokens)
+        decoded, got = _decode_batch(model, engine, tokenizer, head, state, starts, n_tokens, automaton,
+                                     None if init is None else [init[r] for r in rows])
         del state, head
         if verbose > 1:
             print(f"[generate] shared-prompt batch of {len(rows)} rows in {len(parts)} groups, {len(fresh)} prefilled")
@@ -254,19 +289,21 @@ def _generate_shared(prompt_seqs, model, tokenizer, engine, n_tokens, prepend_bo
     return texts, scores
 
 
-def _generate_ragged(prompt_seqs, model, tokenizer, engine, n_tokens, prepend_bos, batch_size, verbose, packed_prefill=False):
+def _generate_ragged(prompt_seqs, model, tokenizer, engine, n_tokens, prepend_bos, batch_size, verbose, packed_prefill=False, automaton=None):
     """generate(ragged=True): prompts sorted by length and cut into batches of <= batch_size; per batch one ragged prefill
     (StripedHyena.prefill_ragged), one first pick (evo_sample) and one on-device loop with per-row positions.  Texts and
     scores come back in input order."""
     from .frontend import ragged_batches
     ids, _ = _ragged_ids(prompt_seqs, model, tokenizer, n_tokens, prepend_bos)
+    init = _initial_states(automaton, ids)
     texts: List[str] = [""] * len(ids)
     scores: List[float] = [0.0] * len(ids)
     for rows, cache_len in ragged_batches([len(t) for t in ids], n_tokens, batch_size):
         with torch.inference_mode():
             head, state = model.prefill_ragged([ids[r] for r in rows], cache_len, packed=packed_prefill)
         starts = torch.tensor([len(ids[r]) for r in rows], dtype=torch.int64)
-        decoded, got = _decode_batch(model, engine, tokenizer, head, state, starts, n_tokens)
+        decoded, got = _decode_batch(model, engine, tokenizer, head, state, starts, n_tokens, automaton,
+                                     None if init is None else [init[r] for r in rows])
         del state, head
         if verbose > 1:
             print(f"[generate] ragged batch of {len(rows)}: prompt lengths {len(ids[rows[0]])}..{len(ids[rows[-1]])}, cache {cache_len}")
@@ -279,7 +316,7 @@ def generate(prompt_seqs: List[str], model, tokenizer: CharLevelTokenizer, n_tok
              top_k: int = 1, top_p: float = 1.0, batched: bool = True, prepend_bos: bool = False,
              cached_generation: bool = False, force_prompt_threshold: int = 128, verbose: int = 1,
              device: str = "cuda:0", ragged: bool = False, batch_size: int = 64, packed_prefill: bool = False, share_prompts: bool = False,
-             **kwargs) -> Tuple[List[str], List[float]]:
+             constraints=None, **kwargs) -> Tuple[List[str], List[float]]:
     """Sequences and mean log-likelihood "scores" for a list of prompts.  Prompts of one common
     length run as one batch; anything else falls back to one prompt at a time (with a note on stderr).
 
@@ -294,7 +331,19 @@ def generate(prompt_seqs: List[str], model, tokenizer: CharLevelTokenizer, n_tok
     share_prompts=True (with ragged=True) draws many samples of a prompt from one prefill: identical prompts form a group,
     each distinct prompt is prefilled once per call, and the group's rows decode against its K,V as one shared prefix
     instead of holding and re-reading a copy each (frontend.shared_batches keeps a group's rows contiguous in batches of at
-    most `batch_size` rows).  Texts and scores come back in input order, scored as with ragged=True."""
+    most `batch_size` rows).  Texts and scores come back in input order, scored as with ragged=True.
+
+    constraints (a constraints.Constraints, with ragged=True) controls what is sampled: only A, C, G and T, none of its
+    forbidden motifs, no homopolymer above its limit, and each row ends at its first (in-frame) stop motif, which is kept.
+    The device sampler masks every pick with the compiled automaton; a row's text ends at its stop, its score is the mean
+    log-likelihood over its kept tokens under the model's unmasked logits, and a batch stops decoding once all its rows
+    have stopped."""
+    if constraints is not None and not ragged:
+        raise ValueError("constraints need ragged=True: the reference-shaped path keeps the reference's sampling")
+    automaton = None
+    if constraints is not None:
+        from .constraints import compile as compile_constraints
+        automaton = compile_constraints(constraints)
     model.eval()
     engine = Generator(model, tokenizer, top_k=top_k, top_p=top_p, temperature=temperature)
     if share_prompts and not ragged:
@@ -305,10 +354,11 @@ def generate(prompt_seqs: List[str], model, tokenizer: CharLevelTokenizer, n_tok
         if batch_size < 1:
             raise ValueError("batch_size must be >= 1")
         if share_prompts:
-            texts, scores = _generate_shared(list(prompt_seqs), model, tokenizer, engine, int(n_tokens), prepend_bos, int(batch_size), verbose)
+            texts, scores = _generate_shared(list(prompt_seqs), model, tokenizer, engine, int(n_tokens), prepend_bos, int(batch_size), verbose,
+                                             automaton=automaton)
         else:
             texts, scores = _generate_ragged(list(prompt_seqs), model, tokenizer, engine, int(n_tokens), prepend_bos, int(batch_size), verbose,
-                                             packed_prefill=bool(packed_prefill))
+                                             packed_prefill=bool(packed_prefill), automaton=automaton)
         if verbose:
             for prompt, text, score in zip(prompt_seqs, texts, scores):
                 print(f'Prompt: "{prompt}",\tOutput: "{text}",\tScore: {score}')

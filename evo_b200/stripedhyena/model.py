@@ -1403,7 +1403,11 @@ class StripedHyena(nn.Module):
         return head, {"mha": mha, "hyena": hy}
 
     # ---- on-device generation loop (SURVEY 8f-2): token pick + bookkeeping + feedback inside the captured step ------
-    def decode_loop(self, first_token, ipd, n_steps, start_pos, *, top_k=1, top_p=0.0, temperature=1.0, forced=None, n_out=None, seed=None):
+    # a constrained loop with stop motifs replays this many steps between reads of its stopped-row counter
+    STOP_CHECK_STEPS = 16
+
+    def decode_loop(self, first_token, ipd, n_steps, start_pos, *, top_k=1, top_p=0.0, temperature=1.0, forced=None, n_out=None, seed=None,
+                    constraints=None):
         """Run `n_steps` single-token steps without returning to the host in between.
 
         first_token (B,) or (B, 1): the input of step 0; ipd: populated state (after a prefill); start_pos: sequence
@@ -1414,7 +1418,14 @@ class StripedHyena(nn.Module):
         Returns (picked (B, n_out) int64, kept_logits (B, n_out, V) fp32) for the sampled steps; the state holders'
         seqlen_offset end at the value the per-token protocol would leave (per-row positions: the largest row's, and the
         attention holder's lengths_per_sample holds every row's).
-        One CUDA graph = one whole step (all blocks + sampler + counters); the host only replays it."""
+        One CUDA graph = one whole step (all blocks + sampler + counters); the host only replays it.
+
+        constraints: a constraints.RowConstraints of the batch.  Its automaton masks every sampled pick and advances each row
+        (evo_sample_step_constrained), and the call returns (picked, kept_logits, lengths), lengths (B,) int64 being each row's
+        generated tokens up to and including its stop motif (-1: not stopped; the loop's first pick is generated token number
+        constraints.index0).  Columns of a stopped row past its length are not written.  When the automaton has stop motifs
+        the loop replays STOP_CHECK_STEPS steps at a time and ends once every row has stopped; the state holders then
+        reflect the steps that ran."""
         lib = _lib.lib()
         dev = self.embedding_layer.weight.device
         x = first_token.reshape(-1, 1).contiguous()
@@ -1465,6 +1476,8 @@ class StripedHyena(nn.Module):
                 pre = mha_ip.prefix_key_value_memory_dict
                 key = ("loop_shared",) + key[1:] + (tuple((pre[i].data_ptr(), tuple(pre[i].shape)) for i in sorted(pre)),
                                                     mha_ip.group_offsets.data_ptr(), mha_ip.prefix_len.data_ptr(), shared["chunks"])
+            if constraints is not None:
+                key = ("constrained",) + key
             st = self._loop
             if st is None or st["key"] != key:
                 st = {"key": key, "graph": None, "x": torch.empty(B, 1, dtype=torch.long, device=dev),
@@ -1473,11 +1486,20 @@ class StripedHyena(nn.Module):
                       "lp_host": torch.zeros(C.sizeof(_lib.LoopParams), dtype=torch.uint8).pin_memory()}
                 if shared is not None:
                     st["spos"] = torch.zeros(B, dtype=torch.int64, device=dev)
+                if constraints is not None:
+                    # the tables and per-row arrays go in through this device-resident struct, so the graph serves every call
+                    st["cp"] = torch.zeros(C.sizeof(_lib.ConstraintParams), dtype=torch.uint8, device=dev)
+                    st["cp_host"] = torch.zeros(C.sizeof(_lib.ConstraintParams), dtype=torch.uint8).pin_memory()
+                    st["stopped_host"] = torch.zeros(1, dtype=torch.int32).pin_memory()
                 self._loop = st
             if st.get("lp_copied") is not None:
                 st["lp_copied"].synchronize()       # a previous call's async copy may not have left the pinned staging buffer yet
             C.memmove(st["lp_host"].data_ptr(), C.addressof(lp), C.sizeof(lp))
             st["lp"].copy_(st["lp_host"], non_blocking=True)
+            if constraints is not None:
+                cp = constraints.params()
+                C.memmove(st["cp_host"].data_ptr(), C.addressof(cp), C.sizeof(cp))
+                st["cp"].copy_(st["cp_host"], non_blocking=True)
             st["lp_copied"] = torch.cuda.Event()
             st["lp_copied"].record()
             if per_row:
@@ -1494,7 +1516,11 @@ class StripedHyena(nn.Module):
                 logits = self._decode_body(st["x"], st["pos"], ipd, B, per_row, shared)
                 prev = lib.evo_set_pdl(int(self.decode_pdl))
                 try:
-                    check(lib.evo_sample_step(ptr(logits), ptr(st["x"]), B, V, ptr(st["lp"]), ptr(st["step"]), self._stream()), "evo_sample_step")
+                    if constraints is None:
+                        check(lib.evo_sample_step(ptr(logits), ptr(st["x"]), B, V, ptr(st["lp"]), ptr(st["step"]), self._stream()), "evo_sample_step")
+                    else:
+                        check(lib.evo_sample_step_constrained(ptr(logits), ptr(st["x"]), B, V, ptr(st["lp"]), ptr(st["cp"]), ptr(st["step"]),
+                                                              self._stream()), "evo_sample_step_constrained")
                     if shared is not None:
                         check(lib.evo_advance_positions(ptr(st["spos"]), B, 1, self._stream()), "evo_advance_positions")
                     if per_row:
@@ -1512,11 +1538,24 @@ class StripedHyena(nn.Module):
                 if self.decode_graph and n_steps > 1:
                     st["graph"], st["launches"], _ = self._capture(one_step)
                     st["ptrs"] = self._graph_ptrs()
-            for _ in range(done, n_steps):
-                if st["graph"] is not None:
-                    self._replay(st)
-                else:
-                    one_step()
+            early_exit = constraints is not None and constraints.automaton.has_stop
+            ran = done
+            while ran < n_steps:
+                n = min(n_steps - ran, self.STOP_CHECK_STEPS) if early_exit else n_steps - ran
+                for _ in range(n):
+                    if st["graph"] is not None:
+                        self._replay(st)
+                    else:
+                        one_step()
+                ran += n
+                if early_exit and ran < n_steps:
+                    st["stopped_host"].copy_(constraints.n_stopped, non_blocking=True)
+                    read = torch.cuda.Event()
+                    read.record()
+                    read.synchronize()
+                    if int(st["stopped_host"][0]) == B:
+                        n_steps = ran
+                        break
             if per_row:
                 mha_ip.lengths_per_sample = (starts + n_steps - 1).to(dev)
                 end = last + n_steps - 1
@@ -1524,7 +1563,10 @@ class StripedHyena(nn.Module):
                 end = int(start_pos) + n_steps - 1          # the position the last step ran at (what the per-token protocol leaves)
             mha_ip.seqlen_offset = hy_ip.seqlen_offset = end
             # the captured graph and its buffers stay alive in self._loop; the outputs are this call's own tensors
-            return picked[:, :n_out], kept[:, :n_out]
+            if constraints is None:
+                return picked[:, :n_out], kept[:, :n_out]
+            constraints.index0 += max(n_steps - n_forced, 0)
+            return picked[:, :n_out], kept[:, :n_out], constraints.length.clone()
 
     def _graph_ptrs(self):
         """Addresses a captured step bakes in besides the state tensors: rope tables, the stream-K workspace and, for an FP8

@@ -356,6 +356,34 @@ int evo_sample_step(const void* logits, int64_t* x, int B, int V, const evo_loop
                     const int64_t* step_dev, void* stream);
 int evo_advance_counters(int64_t* a, int64_t* b, int64_t delta, void* stream);
 
+/* ---- constrained sampling: a deterministic automaton over {A, C, G, T} (evo_b200/constraints.py compiles it) restricts
+ * which tokens each row may pick and ends rows at stop motifs ----
+ * Token t may be picked in state s when 0 <= t < n_tokens, token_symbol[t] >= 0 and bit token_symbol[t] of allow[s] is set.
+ * The distribution is evo_sample's on logits whose disallowed entries are -inf: allowed entries take the first ranks
+ * (non-NaN by value, then NaN), so top-k counts allowed tokens, and when no allowed entry carries weight the pick is the
+ * allowed entry of rank 0.  A table that allows every token gives evo_sample's / evo_sample_step's picks bit for bit.
+ * After a pick with generated index g a running row (length[row] < 0) moves to s' = next[s][symbol]; when stop[s'] is set
+ * length[row] = g + 1 and *n_stopped is incremented, once per row.  A stopped row is neither sampled nor advanced: out /
+ * picked / kept_logits are not written for it and x[row] keeps its last token.  Everything here lives in DEVICE memory.
+ * evo_sample_constrained: evo_sample under the automaton; its pick has generated index index0.
+ * evo_sample_step_constrained: evo_sample_step under the automaton; forced steps do not touch it, and the pick of step i
+ *   has generated index index0 + i - n_forced. */
+typedef struct {
+  const int32_t* next;           /* (n_states, 4) successor per symbol A, C, G, T */
+  const uint8_t* allow;          /* (n_states) bit a set: symbol a may be picked */
+  const uint8_t* stop;           /* (n_states) nonzero: reaching the state ends the row */
+  const int8_t* token_symbol;    /* (n_tokens) symbol of each token, -1: never picked */
+  int32_t n_states; int32_t n_tokens;
+  int32_t* state;                /* (B) per-row state */
+  int64_t* length;               /* (B) -1 while the row runs, then its generated tokens including the stop motif */
+  int32_t* n_stopped;            /* rows stopped so far */
+  int64_t index0;
+} evo_constraint_params;
+int evo_sample_constrained(const void* logits, int64_t* out, int B, int V, int top_k, float top_p, float temperature,
+                           uint64_t seed, uint64_t step, const evo_constraint_params* constraint_params_dev, void* stream);
+int evo_sample_step_constrained(const void* logits, int64_t* x, int B, int V, const evo_loop_params* loop_params_dev,
+                                const evo_constraint_params* constraint_params_dev, const int64_t* step_dev, void* stream);
+
 /* (test comparators -- cuBLASLt GEMM, CUDA-core attention, bf16 add -- live in tests/support/libevo_b200_test.so,
  *  not in this library) */
 

@@ -19,12 +19,14 @@ sampling: each distinct prompt is prefilled once and its samples decode against 
 flags keep the reference's `type=bool` parsing (any non-empty value is True).  --fp8-weights generates with an FP8-weight
 model (Evo(weights="fp8")); scripts/score.py --fp8-weights scores under the same model.  --fp8-compact uses the same FP8
 model holding only its one-byte weights (Evo(weights="fp8-compact")): the same tokens in about half the bf16 weight memory.
+--acgt-only, --forbid, --max-homopolymer, --stop and --stop-in-frame constrain what is sampled (evo_b200.Constraints): any of
+them keeps the outputs to A, C, G and T; they need the ragged paths (--prompts-csv or --share-prompts).
 """
 import argparse
 
 import torch
 
-from evo_b200 import Evo, generate
+from evo_b200 import Constraints, Evo, generate
 from evo_b200.frontend import read_prompts_csv
 
 
@@ -56,7 +58,26 @@ def build_parser():
     parser.add_argument('--samples-per-prompt', type=int, default=1, help='Samples of each --prompts-csv prompt, prompt-major')
     parser.add_argument('--share-prompts', action='store_true',
                         help='Prefill each distinct prompt once and decode its samples against one shared K,V prefix')
+    parser.add_argument('--acgt-only', action='store_true', help='Sample only the bytes A, C, G and T')
+    parser.add_argument('--forbid', type=str, default=None,
+                        help='Comma-separated motifs that must not appear in the output, on either strand (e.g. GGTCTC,CGTCTC)')
+    parser.add_argument('--max-homopolymer', type=int, default=None, help='Longest run of one base allowed in the output')
+    parser.add_argument('--stop', type=str, default=None,
+                        help='Comma-separated motifs that end a sample when generated (e.g. TAA,TAG,TGA); the motif is kept')
+    parser.add_argument('--stop-in-frame', action='store_true',
+                        help='--stop motifs count only at codon boundaries, counted from the prompt\'s first nucleotide')
     return parser
+
+
+def constraints_arg(args):
+    """The Constraints the constraint flags describe, or None when none is given."""
+    split = lambda v: tuple(m.strip() for m in v.split(',') if m.strip()) if v else ()
+    if not (args.acgt_only or args.forbid or args.max_homopolymer is not None or args.stop or args.stop_in_frame):
+        return None
+    if args.prompts_csv is None and not args.share_prompts:
+        raise SystemExit('constraint flags need --prompts-csv or --share-prompts')
+    return Constraints(forbid=split(args.forbid), max_homopolymer=args.max_homopolymer, stop=split(args.stop),
+                       stop_in_frame=args.stop_in_frame)
 
 
 def weights_arg(args):
@@ -66,6 +87,7 @@ def weights_arg(args):
 
 def main(argv=None):
     args = build_parser().parse_args(argv)
+    constraints = constraints_arg(args)
     evo_model = Evo(args.model_name, device=args.device, random_init=args.random_init, model_dir=args.model_dir,
                     weights=weights_arg(args))
     model, tokenizer = evo_model.model, evo_model.tokenizer
@@ -79,11 +101,12 @@ def main(argv=None):
         prompts = [p for p in read_prompts_csv(args.prompts_csv) for _ in range(args.samples_per_prompt)]
         return generate(prompts, model, tokenizer, n_tokens=args.n_tokens, temperature=args.temperature,
                         top_k=args.top_k, top_p=args.top_p, cached_generation=True, prepend_bos=args.prepend_bos, device=args.device,
-                        verbose=args.verbose, ragged=True, batch_size=args.batch_size, share_prompts=args.share_prompts)
+                        verbose=args.verbose, ragged=True, batch_size=args.batch_size, share_prompts=args.share_prompts,
+                        constraints=constraints)
     if args.share_prompts:
         return generate([args.prompt] * args.n_samples, model, tokenizer, n_tokens=args.n_tokens, temperature=args.temperature,
                         top_k=args.top_k, top_p=args.top_p, cached_generation=True, prepend_bos=args.prepend_bos, device=args.device,
-                        verbose=args.verbose, ragged=True, batch_size=args.batch_size, share_prompts=True)
+                        verbose=args.verbose, ragged=True, batch_size=args.batch_size, share_prompts=True, constraints=constraints)
     return generate([args.prompt] * args.n_samples, model, tokenizer, n_tokens=args.n_tokens, temperature=args.temperature,
                     top_k=args.top_k, top_p=args.top_p, cached_generation=args.cached_generation, batched=args.batched,
                     prepend_bos=args.prepend_bos, device=args.device, verbose=args.verbose)
